@@ -31,7 +31,7 @@ extern "C" {
 #define SAE_E_UNSUPPORTED  -3   /* valid request this build has no kernel for                */
 
 /* ABI version of this header; bumped on any signature change. */
-#define SAE_ABI_VERSION 13
+#define SAE_ABI_VERSION 14
 int         sae_abi_version(void);
 const char* sae_last_error(void);
 /* number of kernels launched by this library in the calling process since load
@@ -236,6 +236,24 @@ int sae_conv2d_wgrad(const float* dy, const float* x, float* dw, const sae_conv_
 int sae_conv2d_query_impl(const sae_conv_geom* g, int dir);
 
 /* ------------------------------------------------------------------------------------------
+ * fp32-accurate ("split-TF32", 3xTF32) convolutions.  The entry points above consume their operands at TF32 precision (the
+ * tensor cores ignore the low 13 mantissa bits).  The _3xtf32 twins below split every operand v into hi = rna_tf32(v) and
+ * lo = rna_tf32(v - hi) and form a*b ~= a_hi*b_hi + a_hi*b_lo + a_lo*b_hi on the TF32 tensor cores with fp32 accumulators
+ * (a_lo*b_lo, below fp32 rounding, is dropped): about 22 significant bits per operand at three tensor-core products per pair.
+ * Activations are split inside the kernels; the filter arrives pre-split as the pair (w_hi, w_lo) = sae_split_tf32(w), in the
+ * layout of the TF32 entry point's filter.  Geometry, epilogue, impl (0 auto, 1 generic, 2 wgmma) and eligibility are those
+ * of the TF32 twin; callers that want fp32 results pass epi->round_tf32 = 0 and unrounded operands.
+ * sae_split_tf32: hi[i] = rna_tf32(x[i]), lo[i] = rna_tf32(x[i] - hi[i]) for any contiguous filter tensor, including the
+ * per-sample [N,K,R,S,C] / [N,C,R,S,K] ones of sae_filter_modulate.
+ * ------------------------------------------------------------------------------------------ */
+int sae_split_tf32(const float* x, float* hi, float* lo, int64_t n, void* stream);
+int sae_conv2d_fprop_3xtf32(const float* x, const float* w_hi, const float* w_lo, float* y, const sae_conv_geom* g,
+                            const sae_conv_epilogue* epi, int impl, void* stream);
+int sae_conv2d_dgrad_3xtf32(const float* dy, const float* wt_hi, const float* wt_lo, float* dx, const sae_conv_geom* g,
+                            const sae_conv_epilogue* epi, int impl, void* stream);
+int sae_conv2d_wgrad_3xtf32(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Data-parallel gradient exchange helpers (SURVEY.md §8(e)): pack the active parameter group's
  * gradients into one flat fp32 bucket for a single NCCL all-reduce, then unpack scaled by 1/world.
  * Replaces nn.DataParallel's ReduceAddCoalesced onto GPU 0 (models/__init__.py:80).
@@ -269,6 +287,14 @@ int sae_conv2d_dgrad_per_sample(const float* dy, const float* w_ncrsk, float* dx
                                 const sae_conv_epilogue* epi, void* stream);
 int sae_conv2d_wgrad_modulated(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
                                const sae_conv_geom* g, void* stream);
+/* split-TF32 twins (see sae_conv2d_fprop_3xtf32): per-sample filters as (hi, lo) pairs; the modulated weight gradient
+ * splits dy and x in-kernel and takes the arguments of sae_conv2d_wgrad_modulated */
+int sae_conv2d_fprop_per_sample_3xtf32(const float* x, const float* w_nkrsc_hi, const float* w_nkrsc_lo, float* y,
+                                       const sae_conv_geom* g, const sae_conv_epilogue* epi, void* stream);
+int sae_conv2d_dgrad_per_sample_3xtf32(const float* dy, const float* w_ncrsk_hi, const float* w_ncrsk_lo, float* dx,
+                                       const sae_conv_geom* g, const sae_conv_epilogue* epi, void* stream);
+int sae_conv2d_wgrad_modulated_3xtf32(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
+                                      const sae_conv_geom* g, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Multi-tensor Adam (SURVEY.md §8 f2).  Replaces the two torch.optim.Adam instances of

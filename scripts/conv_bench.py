@@ -1,6 +1,9 @@
 #!/usr/bin/env python
 """Per-shape throughput of the conv kernels (CUDA-event timed, L2 flushed between iterations).
-usage: python scripts/conv_bench.py [--impl 0|1|2] [--dirs fprop,dgrad,wgrad] [--only SUBSTR] [--iters N] [--batch B]"""
+usage: python scripts/conv_bench.py [--impl 0|1|2] [--dirs fprop,dgrad,wgrad] [--only SUBSTR] [--iters N] [--batch B]
+                                   [--precision tf32|fp32]
+--precision fp32 times the split-TF32 (3xTF32) kernels; its fprop / dgrad rows include the filter split (sae_split_tf32).
+The TFLOP/s column counts the convolution's FLOPs once in both modes."""
 import argparse
 import os
 import sys
@@ -41,11 +44,14 @@ def main():
     ap.add_argument("--only", default="")
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--batch", type=int, default=32)
+    ap.add_argument("--precision", default="tf32", choices=backend.PRECISIONS)
     args = ap.parse_args()
     k = backend.kernels()
     k.conv_impl = args.impl
+    k.precision = args.precision
     dev = torch.device("cuda")
     flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)
+    print("precision %s on %s" % (args.precision, torch.cuda.get_device_name()))
     print("%-42s %-6s %5s %9s %9s %8s" % ("shape", "dir", "impl", "ms", "TFLOP/s", "GB/s"))
     for name, h, c, kk, r, stride, pad, mult in SHAPES:
         if args.only and args.only not in name:

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsae_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
 
-SAE_ABI_VERSION = 13
+SAE_ABI_VERSION = 14
 
 c_float_p = ctypes.c_void_p   # raw device pointers travel as integers
 c_stream = ctypes.c_void_p
@@ -87,6 +87,13 @@ SIGNATURES = {
     "sae_conv2d_wgrad": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom), ctypes.c_int,
                                         c_stream]),
     "sae_conv2d_query_impl": (ctypes.c_int, [ctypes.POINTER(ConvGeom), ctypes.c_int]),
+    "sae_split_tf32": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, ctypes.c_int64, c_stream]),
+    "sae_conv2d_fprop_3xtf32": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom),
+                                               ctypes.POINTER(ConvEpilogue), ctypes.c_int, c_stream]),
+    "sae_conv2d_dgrad_3xtf32": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom),
+                                               ctypes.POINTER(ConvEpilogue), ctypes.c_int, c_stream]),
+    "sae_conv2d_wgrad_3xtf32": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom), ctypes.c_int,
+                                               c_stream]),
     "sae_bucket_pack": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, c_float_p,
                                        ctypes.c_int64, c_stream]),
     "sae_bucket_unpack": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, c_float_p,
@@ -98,6 +105,11 @@ SIGNATURES = {
     "sae_conv2d_dgrad_per_sample": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom),
                                                    ctypes.POINTER(ConvEpilogue), c_stream]),
     "sae_conv2d_wgrad_modulated": (ctypes.c_int, [c_float_p] * 6 + [ctypes.POINTER(ConvGeom), c_stream]),
+    "sae_conv2d_fprop_per_sample_3xtf32": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom),
+                                                          ctypes.POINTER(ConvEpilogue), c_stream]),
+    "sae_conv2d_dgrad_per_sample_3xtf32": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom),
+                                                          ctypes.POINTER(ConvEpilogue), c_stream]),
+    "sae_conv2d_wgrad_modulated_3xtf32": (ctypes.c_int, [c_float_p] * 6 + [ctypes.POINTER(ConvGeom), c_stream]),
     "sae_adam_step": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                      c_float_p, c_float_p, c_float_p] + [ctypes.c_float] * 5 + [c_stream]),
     "sae_crop_gather": (ctypes.c_int, [c_float_p] * 5 + [ctypes.c_int] * 7 + [ctypes.c_int64] * 4 + [ctypes.c_int, c_stream]),

@@ -26,6 +26,20 @@ def make_geom(N, H, W, C, K, R, S, stride, pad_t, pad_l, P=None, Q=None):
     return ConvGeom(N, H, W, C, K, R, S, P, Q, stride, pad_t, pad_l)
 
 
+PRECISIONS = ("tf32", "fp32")
+
+
+def parse_precision(value):
+    """``SAE_PRECISION`` / ``CudaKernels.precision`` value -> "tf32" (unset or empty: the default) or "fp32"; anything else
+    raises ValueError"""
+    v = "" if value is None else str(value).strip().lower()
+    if v == "":
+        return "tf32"
+    if v not in PRECISIONS:
+        raise ValueError("unknown precision %r (SAE_PRECISION): expected one of %s" % (value, ", ".join(PRECISIONS)))
+    return v
+
+
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
@@ -108,11 +122,38 @@ class CudaKernels:
         self.conv_impl = 0       # 0 auto, 1 force generic (mma.sync), 2 force wgmma
         # Every activation / gradient / filter this library writes is rounded to the nearest TF32 value (still stored
         # as fp32): the tensor cores ignore the low 13 mantissa bits of their operands, so rounding in the producer
-        # makes that truncation exact and unbiased.  Set False for bit-exact fp32 results from the pointwise kernels.
+        # makes that truncation exact and unbiased.  Set False for bit-exact fp32 results from the pointwise kernels
+        # (the convolutions stay TF32; precision = "fp32" below gives fp32-accurate convolutions).
         self.round_tf32 = True
         self.fused_fir_act = os.environ.get("SAE_FUSED_FIR_ACT", "1") != "0"
         # activation bit masks next to the tensor-core convs' / the FIR + activation kernel's outputs (A/B: SAE_ACT_MASK=0)
         self.act_masks = os.environ.get("SAE_ACT_MASK", "1") != "0"
+        # "tf32" (default): convolutions and linears consume TF32 operands.  "fp32": they run the split-TF32 (3xTF32) kernels,
+        # fp32-accurate products at about a third of the TF32 tensor-core rate, and nothing is rounded to TF32 on storage
+        # (every round_tf32 argument is 0).  The torch flags (cudnn.allow_tf32, matmul.allow_tf32) are not consulted.
+        self.precision = os.environ.get("SAE_PRECISION")
+
+    @property
+    def precision(self):
+        return self._precision
+
+    @precision.setter
+    def precision(self, value):
+        self._precision = parse_precision(value)
+
+    def _round(self, flag=None):
+        """the round_tf32 argument of a kernel call: the policy flag (or an explicit per-call value), always 0 in fp32 mode"""
+        if self._precision == "fp32":
+            return 0
+        return int(self.round_tf32 if flag is None else flag)
+
+    def split_tf32(self, w):
+        """(hi, lo) = (rna_tf32(w), rna_tf32(w - hi)): the filter pair of the split-TF32 conv entry points"""
+        w = w.contiguous()
+        hi, lo = torch.empty_like(w), torch.empty_like(w)
+        with torch.cuda.device(w.device):
+            check(self.lib.sae_split_tf32(_ptr(w), _ptr(hi), _ptr(lo), w.numel(), _stream()), "sae_split_tf32")
+        return hi, lo
 
     # ------------------------------------------------------------------ FIR
     def upfirdn2d(self, x, kernel, up_x, up_y, down_x, down_y, pad_x0, pad_x1, pad_y0, pad_y1, taps=None):
@@ -132,12 +173,12 @@ class CudaKernels:
                 tx = (ctypes.c_float * kw)(*taps[1])
                 with torch.cuda.device(x.device):
                     check(self.lib.sae_upfirdn2d_separable(_ptr(x), ty, tx, _ptr(out), n, h, w, c, kh, kw, up_x, down_x, pad_x0,
-                                                           pad_x1, pad_y0, pad_y1, int(self.round_tf32), _stream()),
+                                                           pad_x1, pad_y0, pad_y1, self._round(), _stream()),
                           "sae_upfirdn2d_separable")
                 return out
         with torch.cuda.device(x.device):
             check(self.lib.sae_upfirdn2d(_ptr(x), _ptr(kernel), _ptr(out), n, h, w, c, kh, kw, up_x, up_y,
-                                         down_x, down_y, pad_x0, pad_x1, pad_y0, pad_y1, int(self.round_tf32), _stream()),
+                                         down_x, down_y, pad_x0, pad_x1, pad_y0, pad_y1, self._round(), _stream()),
                   "sae_upfirdn2d")
         return out
 
@@ -150,7 +191,7 @@ class CudaKernels:
         with torch.cuda.device(x.device):
             check(self.lib.sae_fused_bias_act(_ptr(x), _ptr(bias), _ptr(ref), _ptr(out), x.numel(), 1,
                                               bias.numel() if bias is not None else 1, act, grad, alpha, scale,
-                                              _ptr(noise), _ptr(noise_weight), c, int(self.round_tf32), _stream()),
+                                              _ptr(noise), _ptr(noise_weight), c, self._round(), _stream()),
                   "sae_fused_bias_act")
         return out
 
@@ -163,7 +204,7 @@ class CudaKernels:
         gnw = torch.zeros(1, device=out.device, dtype=out.dtype) if noise is not None else None
         with torch.cuda.device(out.device):
             check(self.lib.sae_bias_act_backward(_ptr(grad_out), _ptr(out), _ptr(gi), _ptr(gb), out.numel(), c,
-                                                 alpha, scale, _ptr(noise), c, _ptr(gnw), int(self.round_tf32), _ptr(mask), _stream()),
+                                                 alpha, scale, _ptr(noise), c, _ptr(gnw), self._round(), _ptr(mask), _stream()),
                   "sae_bias_act_backward")
         return gi, gb, gnw
 
@@ -185,7 +226,7 @@ class CudaKernels:
         tx = (ctypes.c_float * kw)(*taps[1])
         with torch.cuda.device(grad.device):
             rc = self.lib.sae_fir_act_backward(_ptr(grad), ty, tx, _ptr(act_out), _ptr(gi), _ptr(gb), n, h, w, c, kh, kw,
-                                               px0, px1, py0, py1, alpha, scale, int(self.round_tf32), _ptr(mask), _stream())
+                                               px0, px1, py0, py1, alpha, scale, self._round(), _ptr(mask), _stream())
         if rc == -3:            # SAE_E_UNSUPPORTED: e.g. no TMA on this device
             return None
         check(rc, "sae_fir_act_backward")
@@ -208,7 +249,7 @@ class CudaKernels:
         tx = (ctypes.c_float * kw)(*taps[1])
         with torch.cuda.device(x.device):
             rc = self.lib.sae_fir_bias_act(_ptr(x), ty, tx, _ptr(bias), _ptr(noise), _ptr(noise_weight), _ptr(out), n, h, w, c,
-                                           kh, kw, px0, px1, py0, py1, alpha, scale, int(self.round_tf32), _ptr(mask), _stream())
+                                           kh, kw, px0, px1, py0, py1, alpha, scale, self._round(), _ptr(mask), _stream())
         if rc == -3:
             return None
         check(rc, "sae_fir_bias_act")
@@ -222,7 +263,7 @@ class CudaKernels:
         n, h, w, c = x.shape
         out = torch.empty_like(x)
         with torch.cuda.device(x.device):
-            check(self.lib.sae_modulate(_ptr(x), _ptr(s), _ptr(out), n, h * w, c, int(self.round_tf32), _stream()),
+            check(self.lib.sae_modulate(_ptr(x), _ptr(s), _ptr(out), n, h * w, c, self._round(), _stream()),
                   "sae_modulate")
         return out
 
@@ -233,7 +274,7 @@ class CudaKernels:
         ds = torch.zeros_like(s)
         with torch.cuda.device(x.device):
             check(self.lib.sae_modulate_backward(_ptr(dy), _ptr(x), _ptr(s), _ptr(dx), _ptr(ds), n, h * w, c,
-                                                 int(self.round_tf32), _stream()), "sae_modulate_backward")
+                                                 self._round(), _stream()), "sae_modulate_backward")
         return dx, ds
 
     # ------------------------------------------------------- residual merge
@@ -242,7 +283,7 @@ class CudaKernels:
         _need_cuda(a, b)
         out = torch.empty_like(a)
         with torch.cuda.device(a.device):
-            check(self.lib.sae_add_scale(_ptr(a), _ptr(b), _ptr(out), a.numel(), scale, int(self.round_tf32), _stream()),
+            check(self.lib.sae_add_scale(_ptr(a), _ptr(b), _ptr(out), a.numel(), scale, self._round(), _stream()),
                   "sae_add_scale")
         return out
 
@@ -254,7 +295,7 @@ class CudaKernels:
         out = torch.empty_like(res)
         with torch.cuda.device(res.device):
             check(self.lib.sae_upsample2x_add_scale(_ptr(skip), _ptr(res), _ptr(out), n, h, w, c, scale,
-                                                    int(self.round_tf32), _stream()), "sae_upsample2x_add_scale")
+                                                    self._round(), _stream()), "sae_upsample2x_add_scale")
         return out
 
     def upsample2x_backward(self, dy, scale):
@@ -264,7 +305,7 @@ class CudaKernels:
         out = torch.empty((n, oh // 2, ow // 2, c), device=dy.device, dtype=dy.dtype)
         with torch.cuda.device(dy.device):
             check(self.lib.sae_upsample2x_backward(_ptr(dy), _ptr(out), n, oh // 2, ow // 2, c, scale,
-                                                   int(self.round_tf32), _stream()), "sae_upsample2x_backward")
+                                                   self._round(), _stream()), "sae_upsample2x_backward")
         return out
 
     def pad_channels(self, x, c_out):
@@ -277,7 +318,7 @@ class CudaKernels:
         out = torch.empty((n, h, w, c_out), device=x.device, dtype=x.dtype)
         with torch.cuda.device(x.device):
             check(self.lib.sae_pad_channels(_ptr(x), _ptr(out), n, h * w, c, c_out, x.stride(0), x.stride(1), x.stride(3),
-                                            int(self.round_tf32), _stream()), "sae_pad_channels")
+                                            self._round(), _stream()), "sae_pad_channels")
         return out
 
     def reflect_pad(self, x, pads):
@@ -307,7 +348,7 @@ class CudaKernels:
         krsc = torch.empty((k, r, s, c), device=w_oihw.device, dtype=w_oihw.dtype)
         crsk = torch.empty((c, r, s, k), device=w_oihw.device, dtype=w_oihw.dtype) if want_crsk else None
         with torch.cuda.device(w_oihw.device):
-            check(self.lib.sae_filter_prep(_ptr(w_oihw), _ptr(krsc), _ptr(crsk), k, c, r, s, scale, int(self.round_tf32),
+            check(self.lib.sae_filter_prep(_ptr(w_oihw), _ptr(krsc), _ptr(crsk), k, c, r, s, scale, self._round(),
                                            _stream()), "sae_filter_prep")
         return krsc, crsk
 
@@ -323,7 +364,7 @@ class CudaKernels:
     def _filter(self, w):
         """contiguous copy of a (small) filter tensor, rounded to TF32 when the policy says so"""
         w = w.contiguous()
-        if not self.round_tf32:
+        if not self._round():
             return w
         out = torch.empty_like(w)
         with torch.cuda.device(w.device):
@@ -347,7 +388,7 @@ class CudaKernels:
         e.noise_weight = noise_weight.data_ptr() if noise_weight is not None else None
         e.residual = residual.data_ptr() if residual is not None else None
         e.alpha, e.gain, e.res_scale, e.act = alpha, gain, res_scale, act
-        e.round_tf32 = int(self.round_tf32 if round_tf32 is None else round_tf32)
+        e.round_tf32 = self._round(round_tf32)
         e.act_mask = act_mask.data_ptr() if act_mask is not None else None
         return e
 
@@ -365,8 +406,13 @@ class CudaKernels:
             mask = self._new_act_mask(y, 3, impl == 2 or (impl == 0 and self.conv_impl_for(g, 0) == 2))
         e = self._epi(act_mask=mask, **epi)
         with torch.cuda.device(x.device):
-            check(self.lib.sae_conv2d_fprop(_ptr(x), _ptr(w_krsc), _ptr(y), ctypes.byref(g), ctypes.byref(e), impl, _stream()),
-                  "sae_conv2d_fprop")
+            if self._precision == "fp32":
+                hi, lo = self.split_tf32(w_krsc)
+                check(self.lib.sae_conv2d_fprop_3xtf32(_ptr(x), _ptr(hi), _ptr(lo), _ptr(y), ctypes.byref(g), ctypes.byref(e), impl,
+                                                       _stream()), "sae_conv2d_fprop_3xtf32")
+            else:
+                check(self.lib.sae_conv2d_fprop(_ptr(x), _ptr(w_krsc), _ptr(y), ctypes.byref(g), ctypes.byref(e), impl, _stream()),
+                      "sae_conv2d_fprop")
         if mask is not None:
             y._sae_act_mask = mask
         return y
@@ -380,9 +426,15 @@ class CudaKernels:
         wt = w_crsk if w_crsk is not None else self._filter(w_krsc.permute(3, 1, 2, 0))     # [C,R,S,K]
         dx = torch.empty((g.N, g.H, g.W, g.C), device=dy.device, dtype=dy.dtype)
         e = self._epi(**epi)
+        impl = self.conv_impl if impl is None else impl
         with torch.cuda.device(dy.device):
-            check(self.lib.sae_conv2d_dgrad(_ptr(dy), _ptr(wt), _ptr(dx), ctypes.byref(g), ctypes.byref(e),
-                                            self.conv_impl if impl is None else impl, _stream()), "sae_conv2d_dgrad")
+            if self._precision == "fp32":
+                hi, lo = self.split_tf32(wt)
+                check(self.lib.sae_conv2d_dgrad_3xtf32(_ptr(dy), _ptr(hi), _ptr(lo), _ptr(dx), ctypes.byref(g), ctypes.byref(e), impl,
+                                                       _stream()), "sae_conv2d_dgrad_3xtf32")
+            else:
+                check(self.lib.sae_conv2d_dgrad(_ptr(dy), _ptr(wt), _ptr(dx), ctypes.byref(g), ctypes.byref(e), impl, _stream()),
+                      "sae_conv2d_dgrad")
         return dx
 
     def conv_wgrad(self, dy, x, g, impl=None):
@@ -391,9 +443,10 @@ class CudaKernels:
         assert tuple(dy.shape) == (g.N, g.P, g.Q, g.K) and tuple(x.shape) == (g.N, g.H, g.W, g.C), \
             (tuple(dy.shape), tuple(x.shape), g.key())
         dw = torch.zeros((g.K, g.R, g.S, g.C), device=dy.device, dtype=dy.dtype)
+        fn, name = ((self.lib.sae_conv2d_wgrad_3xtf32, "sae_conv2d_wgrad_3xtf32") if self._precision == "fp32"
+                    else (self.lib.sae_conv2d_wgrad, "sae_conv2d_wgrad"))
         with torch.cuda.device(dy.device):
-            check(self.lib.sae_conv2d_wgrad(_ptr(dy), _ptr(x), _ptr(dw), ctypes.byref(g),
-                                            self.conv_impl if impl is None else impl, _stream()), "sae_conv2d_wgrad")
+            check(fn(_ptr(dy), _ptr(x), _ptr(dw), ctypes.byref(g), self.conv_impl if impl is None else impl, _stream()), name)
         return dw
 
     # ------------------------------------------------ style-modulated conv, per-sample filters
@@ -409,7 +462,7 @@ class CudaKernels:
         a = torch.empty((n, k, r, s_, c), device=s.device, dtype=s.dtype) if want_krsc else None
         b = torch.empty((n, c, r, s_, k), device=s.device, dtype=s.dtype) if want_crsk else None
         with torch.cuda.device(s.device):
-            check(self.lib.sae_filter_modulate(_ptr(w_krsc), _ptr(s), _ptr(a), _ptr(b), n, k, c, r, s_, int(self.round_tf32),
+            check(self.lib.sae_filter_modulate(_ptr(w_krsc), _ptr(s), _ptr(a), _ptr(b), n, k, c, r, s_, self._round(),
                                                _stream()), "sae_filter_modulate")
         return a, b
 
@@ -420,8 +473,13 @@ class CudaKernels:
         mask = self._new_act_mask(y, epi.get("act", 1), True)          # only the wgmma kernel implements per-sample filters
         e = self._epi(act_mask=mask, **epi)
         with torch.cuda.device(x.device):
-            check(self.lib.sae_conv2d_fprop_per_sample(_ptr(x), _ptr(w_nkrsc), _ptr(y), ctypes.byref(g), ctypes.byref(e), _stream()),
-                  "sae_conv2d_fprop_per_sample")
+            if self._precision == "fp32":
+                hi, lo = self.split_tf32(w_nkrsc)
+                check(self.lib.sae_conv2d_fprop_per_sample_3xtf32(_ptr(x), _ptr(hi), _ptr(lo), _ptr(y), ctypes.byref(g),
+                                                                  ctypes.byref(e), _stream()), "sae_conv2d_fprop_per_sample_3xtf32")
+            else:
+                check(self.lib.sae_conv2d_fprop_per_sample(_ptr(x), _ptr(w_nkrsc), _ptr(y), ctypes.byref(g), ctypes.byref(e),
+                                                           _stream()), "sae_conv2d_fprop_per_sample")
         if mask is not None:
             y._sae_act_mask = mask
         return y
@@ -432,8 +490,13 @@ class CudaKernels:
         dx = torch.empty((g.N, g.H, g.W, g.C), device=dy.device, dtype=dy.dtype)
         e = self._epi(**epi)
         with torch.cuda.device(dy.device):
-            check(self.lib.sae_conv2d_dgrad_per_sample(_ptr(dy), _ptr(w_ncrsk), _ptr(dx), ctypes.byref(g), ctypes.byref(e), _stream()),
-                  "sae_conv2d_dgrad_per_sample")
+            if self._precision == "fp32":
+                hi, lo = self.split_tf32(w_ncrsk)
+                check(self.lib.sae_conv2d_dgrad_per_sample_3xtf32(_ptr(dy), _ptr(hi), _ptr(lo), _ptr(dx), ctypes.byref(g),
+                                                                  ctypes.byref(e), _stream()), "sae_conv2d_dgrad_per_sample_3xtf32")
+            else:
+                check(self.lib.sae_conv2d_dgrad_per_sample(_ptr(dy), _ptr(w_ncrsk), _ptr(dx), ctypes.byref(g), ctypes.byref(e),
+                                                           _stream()), "sae_conv2d_dgrad_per_sample")
         return dx
 
     def conv_wgrad_modulated(self, dy, x, s, w_krsc, g):
@@ -441,9 +504,10 @@ class CudaKernels:
         _need_cuda(dy, x, s, w_krsc)
         dw = torch.zeros((g.K, g.R, g.S, g.C), device=dy.device, dtype=dy.dtype)
         ds = torch.zeros((g.N, g.C), device=dy.device, dtype=dy.dtype)
+        fn, name = ((self.lib.sae_conv2d_wgrad_modulated_3xtf32, "sae_conv2d_wgrad_modulated_3xtf32") if self._precision == "fp32"
+                    else (self.lib.sae_conv2d_wgrad_modulated, "sae_conv2d_wgrad_modulated"))
         with torch.cuda.device(dy.device):
-            check(self.lib.sae_conv2d_wgrad_modulated(_ptr(dy), _ptr(x), _ptr(s), _ptr(w_krsc), _ptr(dw), _ptr(ds), ctypes.byref(g),
-                                                      _stream()), "sae_conv2d_wgrad_modulated")
+            check(fn(_ptr(dy), _ptr(x), _ptr(s), _ptr(w_krsc), _ptr(dw), _ptr(ds), ctypes.byref(g), _stream()), name)
         return dw, ds
 
     def conv_impl_for(self, g, direction):
@@ -487,7 +551,7 @@ class CudaKernels:
         y = torch.empty((n, h, wd, 4), device=x.device, dtype=x.dtype)
         with torch.cuda.device(x.device):
             check(self.lib.sae_torgb_forward(_ptr(x), _ptr(s), _ptr(w), _ptr(bias), _ptr(y), n, h, wd, c, wscale,
-                                             int(self.round_tf32), _stream()), "sae_torgb_forward")
+                                             self._round(), _stream()), "sae_torgb_forward")
         return y
 
     def torgb_backward(self, dy, x, s, w, wscale, want_dx=True, want_gw=True):
@@ -499,7 +563,7 @@ class CudaKernels:
         gw = torch.zeros((n, 3, c), device=x.device, dtype=x.dtype) if want_gw else None
         with torch.cuda.device(x.device):
             check(self.lib.sae_torgb_backward(_ptr(dy), _ptr(x), _ptr(s), _ptr(w), _ptr(dx), _ptr(gw), n, h, wd, c, wscale,
-                                              dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3), int(self.round_tf32),
+                                              dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3), self._round(),
                                               _stream()), "sae_torgb_backward")
         return dx, gw
 
@@ -515,7 +579,7 @@ class CudaKernels:
         assert tuple(out.shape) == (q, size, size, c_pad) and out.is_contiguous()
         with torch.cuda.device(x.device):
             check(self.lib.sae_crop_gather(_ptr(x), _ptr(flip), _ptr(scale), _ptr(offset), _ptr(out), q, num_crops, c, h, w, size,
-                                           c_pad, x.stride(0), x.stride(1), x.stride(2), x.stride(3), int(self.round_tf32),
+                                           c_pad, x.stride(0), x.stride(1), x.stride(2), x.stride(3), self._round(),
                                            _stream()), "sae_crop_gather")
         return out
 

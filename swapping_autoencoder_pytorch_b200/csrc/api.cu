@@ -47,53 +47,86 @@ extern "C" int sae_conv2d_query_impl(const sae_conv_geom* g, int dir) {
     return ok ? 2 : 1;
 }
 
-extern "C" int sae_conv2d_fprop(const float* x, const float* w, float* y, const sae_conv_geom* g,
-                                const sae_conv_epilogue* epi, int impl, void* stream) {
-    int rc = validate_geom(g, "conv2d_fprop");
+// w_lo non-null: the split-TF32 twin (filter pair (w, w_lo)); the TF32 entry points pass nullptr
+static int conv2d_fprop(const float* x, const float* w, const float* w_lo, float* y, const sae_conv_geom* g,
+                        const sae_conv_epilogue* epi, int impl, void* stream, const char* who) {
+    int rc = validate_geom(g, who);
     if (rc) return rc;
     if (g->N == 0) return SAE_OK;
-    if (!x || !w || !y) return fail(SAE_E_INVALID, "conv2d_fprop: null pointer");
+    if (!x || !w || !y) return fail(SAE_E_INVALID, "%s: null pointer", who);
     cudaStream_t st = (cudaStream_t)stream;
     EpiParams e = make_epi(epi);
     const bool tc_ok = tc_available() && tc_fprop_eligible(g);
-    if (impl == 2 && !tc_ok) return fail(SAE_E_UNSUPPORTED, "conv2d_fprop: shape not eligible for the wgmma kernel");
-    if (impl != 1 && tc_ok) return tc_fprop(x, w, y, g, e, st);
+    if (impl == 2 && !tc_ok) return fail(SAE_E_UNSUPPORTED, "%s: shape not eligible for the wgmma kernel", who);
+    if (impl != 1 && tc_ok) return tc_fprop(x, w, y, g, e, st, w_lo);
     GatherParams p;
     p.N = g->N; p.OH = g->P; p.OW = g->Q; p.IH = g->H; p.IW = g->W; p.Cs = g->C; p.R = g->R; p.S = g->S;
     p.SY = g->stride; p.DY = 1; p.OFFY = -g->pad_t; p.OFFX = -g->pad_l; p.DIV = 1;
     p.Ncol = g->K; p.K = g->R * g->S * g->C; p.M = (int64_t)g->N * g->P * g->Q;
-    return conv_gather_dispatch(x, w, y, p, e, st);
+    return conv_gather_dispatch(x, w, y, p, e, st, w_lo);
 }
 
-extern "C" int sae_conv2d_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g,
-                                const sae_conv_epilogue* epi, int impl, void* stream) {
-    int rc = validate_geom(g, "conv2d_dgrad");
+static int conv2d_dgrad(const float* dy, const float* wt, const float* wt_lo, float* dx, const sae_conv_geom* g,
+                        const sae_conv_epilogue* epi, int impl, void* stream, const char* who) {
+    int rc = validate_geom(g, who);
     if (rc) return rc;
     if (g->N == 0) return SAE_OK;
-    if (!dy || !wt || !dx) return fail(SAE_E_INVALID, "conv2d_dgrad: null pointer");
+    if (!dy || !wt || !dx) return fail(SAE_E_INVALID, "%s: null pointer", who);
     cudaStream_t st = (cudaStream_t)stream;
     EpiParams e = make_epi(epi);
     const bool tc_ok = tc_available() && tc_dgrad_eligible(g);
-    if (impl == 2 && !tc_ok) return fail(SAE_E_UNSUPPORTED, "conv2d_dgrad: shape not eligible for the wgmma kernel");
-    if (impl != 1 && tc_ok) return tc_dgrad(dy, wt, dx, g, e, st);
+    if (impl == 2 && !tc_ok) return fail(SAE_E_UNSUPPORTED, "%s: shape not eligible for the wgmma kernel", who);
+    if (impl != 1 && tc_ok) return tc_dgrad(dy, wt, dx, g, e, st, wt_lo);
     GatherParams p;
     p.N = g->N; p.OH = g->H; p.OW = g->W; p.IH = g->P; p.IW = g->Q; p.Cs = g->K; p.R = g->R; p.S = g->S;
     p.SY = 1; p.DY = -1; p.OFFY = g->pad_t; p.OFFX = g->pad_l; p.DIV = g->stride;
     p.Ncol = g->C; p.K = g->R * g->S * g->K; p.M = (int64_t)g->N * g->H * g->W;
-    return conv_gather_dispatch(dy, wt, dx, p, e, st);
+    return conv_gather_dispatch(dy, wt, dx, p, e, st, wt_lo);
+}
+
+static int conv2d_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, void* stream, bool split,
+                        const char* who) {
+    int rc = validate_geom(g, who);
+    if (rc) return rc;
+    if (g->N == 0) return SAE_OK;
+    if (!dy || !x || !dw) return fail(SAE_E_INVALID, "%s: null pointer", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) == 0;
+    if (impl == 2 && !(tc_available() && al && wgrad_wg_eligible(g)))
+        return fail(SAE_E_UNSUPPORTED, "%s: shape not eligible for the wgmma kernel", who);
+    return conv_wgrad(dy, x, dw, g, impl, st, split);
+}
+
+extern "C" int sae_conv2d_fprop(const float* x, const float* w, float* y, const sae_conv_geom* g,
+                                const sae_conv_epilogue* epi, int impl, void* stream) {
+    return conv2d_fprop(x, w, nullptr, y, g, epi, impl, stream, "conv2d_fprop");
+}
+
+extern "C" int sae_conv2d_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g,
+                                const sae_conv_epilogue* epi, int impl, void* stream) {
+    return conv2d_dgrad(dy, wt, nullptr, dx, g, epi, impl, stream, "conv2d_dgrad");
 }
 
 extern "C" int sae_conv2d_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g,
                                 int impl, void* stream) {
-    int rc = validate_geom(g, "conv2d_wgrad");
-    if (rc) return rc;
-    if (g->N == 0) return SAE_OK;
-    if (!dy || !x || !dw) return fail(SAE_E_INVALID, "conv2d_wgrad: null pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) == 0;
-    if (impl == 2 && !(tc_available() && al && wgrad_wg_eligible(g)))
-        return fail(SAE_E_UNSUPPORTED, "conv2d_wgrad: shape not eligible for the wgmma kernel");
-    return conv_wgrad(dy, x, dw, g, impl, st);
+    return conv2d_wgrad(dy, x, dw, g, impl, stream, false, "conv2d_wgrad");
+}
+
+// ---- split-TF32 (fp32-accurate) twins --------------------------------------------------------------------------------------
+extern "C" int sae_conv2d_fprop_3xtf32(const float* x, const float* w_hi, const float* w_lo, float* y, const sae_conv_geom* g,
+                                       const sae_conv_epilogue* epi, int impl, void* stream) {
+    if (!w_lo && g && g->N > 0) return fail(SAE_E_INVALID, "conv2d_fprop_3xtf32: null pointer");
+    return conv2d_fprop(x, w_hi, w_lo, y, g, epi, impl, stream, "conv2d_fprop_3xtf32");
+}
+
+extern "C" int sae_conv2d_dgrad_3xtf32(const float* dy, const float* wt_hi, const float* wt_lo, float* dx, const sae_conv_geom* g,
+                                       const sae_conv_epilogue* epi, int impl, void* stream) {
+    if (!wt_lo && g && g->N > 0) return fail(SAE_E_INVALID, "conv2d_dgrad_3xtf32: null pointer");
+    return conv2d_dgrad(dy, wt_hi, wt_lo, dx, g, epi, impl, stream, "conv2d_dgrad_3xtf32");
+}
+
+extern "C" int sae_conv2d_wgrad_3xtf32(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, void* stream) {
+    return conv2d_wgrad(dy, x, dw, g, impl, stream, true, "conv2d_wgrad_3xtf32");
 }
 
 // ---- style-modulated convolution with per-sample filters (no modulated copy of the activation) --------------------------
@@ -129,4 +162,33 @@ extern "C" int sae_conv2d_wgrad_modulated(const float* dy, const float* x, const
     if (g->N == 0) return SAE_OK;
     if (!dy || !x || !s || !w_krsc || !dw || !ds) return fail(SAE_E_INVALID, "conv2d_wgrad_modulated: null pointer");
     return conv_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, (cudaStream_t)stream);
+}
+
+extern "C" int sae_conv2d_fprop_per_sample_3xtf32(const float* x, const float* w_nkrsc_hi, const float* w_nkrsc_lo, float* y,
+                                                  const sae_conv_geom* g, const sae_conv_epilogue* epi, void* stream) {
+    int rc = validate_geom(g, "conv2d_fprop_per_sample_3xtf32");
+    if (rc) return rc;
+    if (g->N == 0) return SAE_OK;
+    if (!x || !w_nkrsc_hi || !w_nkrsc_lo || !y) return fail(SAE_E_INVALID, "conv2d_fprop_per_sample_3xtf32: null pointer");
+    if (!tc_available()) return fail(SAE_E_UNSUPPORTED, "conv2d_fprop_per_sample_3xtf32: needs the wgmma path");
+    return tc_conv_per_sample(x, w_nkrsc_hi, y, g, 0, make_epi(epi), (cudaStream_t)stream, w_nkrsc_lo);
+}
+
+extern "C" int sae_conv2d_dgrad_per_sample_3xtf32(const float* dy, const float* w_ncrsk_hi, const float* w_ncrsk_lo, float* dx,
+                                                  const sae_conv_geom* g, const sae_conv_epilogue* epi, void* stream) {
+    int rc = validate_geom(g, "conv2d_dgrad_per_sample_3xtf32");
+    if (rc) return rc;
+    if (g->N == 0) return SAE_OK;
+    if (!dy || !w_ncrsk_hi || !w_ncrsk_lo || !dx) return fail(SAE_E_INVALID, "conv2d_dgrad_per_sample_3xtf32: null pointer");
+    if (!tc_available()) return fail(SAE_E_UNSUPPORTED, "conv2d_dgrad_per_sample_3xtf32: needs the wgmma path");
+    return tc_conv_per_sample(dy, w_ncrsk_hi, dx, g, 1, make_epi(epi), (cudaStream_t)stream, w_ncrsk_lo);
+}
+
+extern "C" int sae_conv2d_wgrad_modulated_3xtf32(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw,
+                                                 float* ds, const sae_conv_geom* g, void* stream) {
+    int rc = validate_geom(g, "conv2d_wgrad_modulated_3xtf32");
+    if (rc) return rc;
+    if (g->N == 0) return SAE_OK;
+    if (!dy || !x || !s || !w_krsc || !dw || !ds) return fail(SAE_E_INVALID, "conv2d_wgrad_modulated_3xtf32: null pointer");
+    return conv_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, (cudaStream_t)stream, true);
 }

@@ -45,6 +45,14 @@ __device__ __forceinline__ float rna_tf32(float v) {
     return __uint_as_float(r);
 }
 
+// split-TF32 ("3xTF32") operand: v ~= hi + lo with hi = rna_tf32(v), lo = rna_tf32(v - hi) (v - hi is exact in fp32), so
+// a*b ~= a_hi b_hi + a_hi b_lo + a_lo b_hi on the TF32 tensor cores carries about 22 significant bits per operand
+__device__ __forceinline__ void split_tf32(float v, uint32_t& hi, uint32_t& lo) {
+    const float h = rna_tf32(v);
+    hi = __float_as_uint(h);
+    lo = __float_as_uint(rna_tf32(v - h));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

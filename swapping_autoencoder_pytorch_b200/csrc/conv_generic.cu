@@ -13,6 +13,9 @@
 // wgrad:  dW[o, (r,s,c)] += sum_pixels dy[pixel, o] * x_gathered[pixel, (r,s,c)], split over pixels,
 //   fp32 atomics into dW.
 // Operands are rounded to TF32 (cvt.rna) when fragments are loaded, accumulation is fp32.
+// Split-TF32 (SPLIT = true, the fp32 precision mode): the activation operands are split into hi = rna_tf32(v),
+// lo = rna_tf32(v - hi) in registers, the gather kernel's filter arrives as the pair (wmat = hi, wlo = lo), and every
+// fragment pair issues three mma (lo*hi + hi*lo + hi*hi).
 #include "conv_internal.cuh"
 
 namespace sae {
@@ -39,14 +42,30 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
+// split-TF32 product of one fragment pair, acc += a b with a = ah + al, b = bh + bl.  The tensor core adds into its
+// accumulator rounding toward zero, a bias that over a long K reaches ~1e-5 relative; so the three products go into a fresh
+// fragment and reach acc through round-to-nearest fp32 adds.
+__device__ __forceinline__ void mma_tf32_3x(float (&acc)[4], const uint32_t (&ah)[4], const uint32_t (&al)[4],
+                                            const uint32_t (&bh)[2], const uint32_t (&bl)[2]) {
+    float t[4];
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%10,%10,%10,%10};"
+                 : "=f"(t[0]), "=f"(t[1]), "=f"(t[2]), "=f"(t[3])
+                 : "r"(al[0]), "r"(al[1]), "r"(al[2]), "r"(al[3]), "r"(bh[0]), "r"(bh[1]), "f"(0.f));
+    mma_tf32(t, ah, bl);
+    mma_tf32(t, ah, bh);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[q] += t[q];
+}
+
 // ------------------------------------------------------------------------------------------------
-template <int BN, bool VEC>
+template <int BN, bool VEC, bool SPLIT>
 __global__ void __launch_bounds__(NTHREADS)
 conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat, float* __restrict__ out,
-                   GatherParams p, EpiParams e) {
+                   GatherParams p, EpiParams e, const float* __restrict__ wlo) {
     extern __shared__ __align__(16) float smem[];
     float* As = smem;                               // [STAGES][BM][LDS_K]
     float* Bs = smem + STAGES * BM * LDS_K;         // [STAGES][BN][LDS_K]
+    float* Bl = Bs + STAGES * BN * LDS_K;           // SPLIT: [STAGES][BN][LDS_K], the filter's low halves
 
     constexpr int WARPS_N = BN / 32;
     constexpr int WARPS_M = 8 / WARPS_N;
@@ -92,6 +111,7 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
         const int kb = kb_begin + kb_rel;
         float* as = As + stage * BM * LDS_K;
         float* bs = Bs + stage * BN * LDS_K;
+        float* bl = Bl + stage * BN * LDS_K;
         if (VEC) {
             const int kq = tid & 7;
             const int k = kb * BK + kq * 4;
@@ -119,6 +139,7 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
                 bool ok = kok && n < p.Ncol;
                 const float* gp = ok ? wmat + (int64_t)n * p.K + k : wmat;
                 cp_async16(bs + row * LDS_K + kq * 4, gp, ok);
+                if constexpr (SPLIT) cp_async16(bl + row * LDS_K + kq * 4, ok ? wlo + (int64_t)n * p.K + k : wlo, ok);
             }
         } else {
             // scalar path (channel counts that are not multiples of 4): plain loads
@@ -151,6 +172,7 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
                 float v = 0.f;
                 if (k < p.K && n < p.Ncol) v = __ldg(wmat + (int64_t)n * p.K + k);
                 bs[row * LDS_K + kk] = v;
+                if constexpr (SPLIT) bl[row * LDS_K + kk] = (k < p.K && n < p.Ncol) ? __ldg(wlo + (int64_t)n * p.K + k) : 0.f;
             }
         }
     };
@@ -178,6 +200,34 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
         }
         const float* as = As + (kb % STAGES) * BM * LDS_K + (wm * WM) * LDS_K;
         const float* bs = Bs + (kb % STAGES) * BN * LDS_K + (wn * 32) * LDS_K;
+        if constexpr (SPLIT) {
+            const float* bl = Bl + (kb % STAGES) * BN * LDS_K + (wn * 32) * LDS_K;
+#pragma unroll
+            for (int ks = 0; ks < BK / 8; ++ks) {
+                uint32_t ah[MT][4], al[MT][4], bh[NT][2], blo[NT][2];
+#pragma unroll
+                for (int i = 0; i < MT; ++i) {
+                    const float* a = as + (i * 16 + g) * LDS_K + ks * 8 + t;
+                    split_tf32(a[0], ah[i][0], al[i][0]);
+                    split_tf32(a[8 * LDS_K], ah[i][1], al[i][1]);
+                    split_tf32(a[4], ah[i][2], al[i][2]);
+                    split_tf32(a[8 * LDS_K + 4], ah[i][3], al[i][3]);
+                }
+#pragma unroll
+                for (int j = 0; j < NT; ++j) {
+                    const int o = (j * 8 + g) * LDS_K + ks * 8 + t;
+                    bh[j][0] = __float_as_uint(bs[o]);
+                    bh[j][1] = __float_as_uint(bs[o + 4]);
+                    blo[j][0] = __float_as_uint(bl[o]);
+                    blo[j][1] = __float_as_uint(bl[o + 4]);
+                }
+#pragma unroll
+                for (int i = 0; i < MT; ++i)
+#pragma unroll
+                    for (int j = 0; j < NT; ++j) mma_tf32_3x(acc[i][j], ah[i], al[i], bh[j], blo[j]);
+            }
+            continue;
+        }
 #pragma unroll
         for (int ks = 0; ks < BK / 8; ++ks) {
             uint32_t af[MT][4], bf[NT][2];
@@ -282,7 +332,7 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
 // ------------------------------------------------------------------------------------------------
 constexpr int LDS_M = 128 + 8;
 
-template <bool VA, bool VB>
+template <bool VA, bool VB, bool SPLIT>
 __global__ void __launch_bounds__(NTHREADS)
 conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, float* __restrict__ dw, WgradParams p) {
     extern __shared__ __align__(16) float smem[];
@@ -400,6 +450,31 @@ conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, flo
         }
         const float* as = As + (kb % STAGES) * BK * LDS_M + wm * 64;
         const float* bs = Bs + (kb % STAGES) * BK * LDS_M + wn * 32;
+        if constexpr (SPLIT) {
+#pragma unroll
+            for (int ks = 0; ks < BK / 8; ++ks) {
+                uint32_t ah[4][4], al[4][4], bh[4][2], blo[4][2];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float* a = as + (ks * 8 + t) * LDS_M + i * 16 + g;
+                    split_tf32(a[0], ah[i][0], al[i][0]);
+                    split_tf32(a[8], ah[i][1], al[i][1]);
+                    split_tf32(a[4 * LDS_M], ah[i][2], al[i][2]);
+                    split_tf32(a[4 * LDS_M + 8], ah[i][3], al[i][3]);
+                }
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float* b = bs + (ks * 8 + t) * LDS_M + j * 8 + g;
+                    split_tf32(b[0], bh[j][0], blo[j][0]);
+                    split_tf32(b[4 * LDS_M], bh[j][1], blo[j][1]);
+                }
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) mma_tf32_3x(acc[i][j], ah[i], al[i], bh[j], blo[j]);
+            }
+            continue;
+        }
 #pragma unroll
         for (int ks = 0; ks < BK / 8; ++ks) {
             uint32_t af[4][4], bf[4][2];
@@ -471,13 +546,13 @@ conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, flo
 }
 
 // ------------------------------------------------------------------------------------------------
-template <int BN, bool VEC>
+template <int BN, bool VEC, bool SPLIT>
 static int launch_gather(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
-                         cudaStream_t st) {
-    size_t smem = (size_t)STAGES * (BM + BN) * LDS_K * sizeof(float);
+                         cudaStream_t st, const float* wlo) {
+    size_t smem = (size_t)STAGES * (BM + (SPLIT ? 2 : 1) * BN) * LDS_K * sizeof(float);
     static bool attr_done = false;   // benign race: idempotent
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_gather_kernel<BN, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_gather_kernel<BN, VEC, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done = true;
     }
     dim3 grid((unsigned)((p.M + BM - 1) / BM), (unsigned)((p.Ncol + BN - 1) / BN));
@@ -492,35 +567,52 @@ static int launch_gather(const float* src, const float* wmat, float* out, const 
             SAE_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)p.M * p.Ncol * sizeof(float), st));
         }
     }
-    conv_gather_kernel<BN, VEC><<<grid, NTHREADS, smem, st>>>(src, wmat, out, p, e);
+    conv_gather_kernel<BN, VEC, SPLIT><<<grid, NTHREADS, smem, st>>>(src, wmat, out, p, e, wlo);
     return check_launch("conv_gather");
 }
 
-int conv_gather_dispatch(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
-                         cudaStream_t st) {
-    if (p.M == 0 || p.Ncol == 0) return SAE_OK;
-    const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(wmat)) & 15) == 0;
+template <bool SPLIT>
+static int gather_dispatch_t(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
+                             cudaStream_t st, const float* wlo) {
+    const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(wmat) | reinterpret_cast<uintptr_t>(wlo)) & 15) == 0;
     const bool vec = (p.Cs % 4 == 0) && aligned;
-    if (p.Ncol > 64) return vec ? launch_gather<128, true>(src, wmat, out, p, e, st) : launch_gather<128, false>(src, wmat, out, p, e, st);
-    if (p.Ncol > 32) return vec ? launch_gather<64, true>(src, wmat, out, p, e, st) : launch_gather<64, false>(src, wmat, out, p, e, st);
-    return vec ? launch_gather<32, true>(src, wmat, out, p, e, st) : launch_gather<32, false>(src, wmat, out, p, e, st);
+    if (p.Ncol > 64)
+        return vec ? launch_gather<128, true, SPLIT>(src, wmat, out, p, e, st, wlo) : launch_gather<128, false, SPLIT>(src, wmat, out, p, e, st, wlo);
+    if (p.Ncol > 32)
+        return vec ? launch_gather<64, true, SPLIT>(src, wmat, out, p, e, st, wlo) : launch_gather<64, false, SPLIT>(src, wmat, out, p, e, st, wlo);
+    return vec ? launch_gather<32, true, SPLIT>(src, wmat, out, p, e, st, wlo) : launch_gather<32, false, SPLIT>(src, wmat, out, p, e, st, wlo);
 }
 
-template <bool VA, bool VB>
+int conv_gather_dispatch(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
+                         cudaStream_t st, const float* wlo) {
+    if (p.M == 0 || p.Ncol == 0) return SAE_OK;
+    return wlo ? gather_dispatch_t<true>(src, wmat, out, p, e, st, wlo) : gather_dispatch_t<false>(src, wmat, out, p, e, st, nullptr);
+}
+
+template <bool VA, bool VB, bool SPLIT>
 static int launch_wgrad(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st) {
     size_t smem = (size_t)STAGES * 2 * BK * LDS_M * sizeof(float);
     static bool attr_done = false;
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_wgrad_kernel<VA, VB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_wgrad_kernel<VA, VB, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done = true;
     }
     dim3 grid((unsigned)((p.Ko + 127) / 128), (unsigned)((p.Ncol + 127) / 128), splits);
-    conv_wgrad_kernel<VA, VB><<<grid, NTHREADS, smem, st>>>(dy, x, dw, p);
+    conv_wgrad_kernel<VA, VB, SPLIT><<<grid, NTHREADS, smem, st>>>(dy, x, dw, p);
     return check_launch("conv_wgrad");
 }
 
+template <bool SPLIT>
+static int launch_wgrad_any(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st,
+                            bool va, bool vb) {
+    if (va && vb) return launch_wgrad<true, true, SPLIT>(dy, x, dw, p, splits, st);
+    if (va) return launch_wgrad<true, false, SPLIT>(dy, x, dw, p, splits, st);
+    if (vb) return launch_wgrad<false, true, SPLIT>(dy, x, dw, p, splits, st);
+    return launch_wgrad<false, false, SPLIT>(dy, x, dw, p, splits, st);
+}
+
 static int wgrad_impl(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st,
-                      const float* mod_s, const float* mod_w, float* mod_ds) {
+                      const float* mod_s, const float* mod_w, float* mod_ds, bool split) {
     WgradParams p;
     p.mod_s = mod_s; p.mod_w = mod_w; p.mod_ds = mod_ds;
     p.img_pix = mod_s ? (int64_t)g->P * g->Q : 0;
@@ -542,15 +634,12 @@ static int wgrad_impl(const float* dy, const float* x, float* dw, const sae_conv
     unsigned splits = (unsigned)((p.Mpix + p.chunk - 1) / p.chunk);
     const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) == 0;
     const bool va = (p.Ko % 4 == 0) && al, vb = (p.C % 4 == 0) && al;
-    if (impl != 1 && va && vb && tc_available()) return wgrad_wg_launch(dy, x, dw, p, splits, st);
-    if (va && vb) return launch_wgrad<true, true>(dy, x, dw, p, splits, st);
-    if (va) return launch_wgrad<true, false>(dy, x, dw, p, splits, st);
-    if (vb) return launch_wgrad<false, true>(dy, x, dw, p, splits, st);
-    return launch_wgrad<false, false>(dy, x, dw, p, splits, st);
+    if (impl != 1 && va && vb && tc_available()) return wgrad_wg_launch(dy, x, dw, p, splits, st, split);
+    return split ? launch_wgrad_any<true>(dy, x, dw, p, splits, st, va, vb) : launch_wgrad_any<false>(dy, x, dw, p, splits, st, va, vb);
 }
 
-int conv_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st) {
-    return wgrad_impl(dy, x, dw, g, impl, st, nullptr, nullptr, nullptr);
+int conv_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st, bool split) {
+    return wgrad_impl(dy, x, dw, g, impl, st, nullptr, nullptr, nullptr, split);
 }
 
 bool wgrad_modulated_eligible(const sae_conv_geom* g) {
@@ -560,11 +649,11 @@ bool wgrad_modulated_eligible(const sae_conv_geom* g) {
 }
 
 int conv_wgrad_modulated(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
-                         const sae_conv_geom* g, cudaStream_t st) {
+                         const sae_conv_geom* g, cudaStream_t st, bool split) {
     if (!wgrad_modulated_eligible(g)) return fail(SAE_E_UNSUPPORTED, "modulated wgrad: needs stride 1, Q %% 32 == 0, C and K %% 32 == 0");
     if (((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) != 0)
         return fail(SAE_E_INVALID, "modulated wgrad: pointers must be 16-byte aligned");
-    return wgrad_impl(dy, x, dw, g, 0, st, s, w_krsc, ds);
+    return wgrad_impl(dy, x, dw, g, 0, st, s, w_krsc, ds, split);
 }
 
 }  // namespace sae

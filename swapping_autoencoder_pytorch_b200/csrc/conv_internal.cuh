@@ -32,27 +32,33 @@ struct WgradParams {
     float* mod_ds;        // [N, C], accumulated
 };
 // conv_generic.cu
+// wlo non-null: split-TF32 operands, the filter given as the pair (wmat, wlo) = (hi, lo)
 int conv_gather_dispatch(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
-                         cudaStream_t st);
-// impl: 0 = the wgmma kernel where the channel counts allow it (wgrad_wgmma.cu), 1 = the mma.sync kernel
-int conv_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st);
+                         cudaStream_t st, const float* wlo = nullptr);
+// impl: 0 = the wgmma kernel where the channel counts allow it (wgrad_wgmma.cu), 1 = the mma.sync kernel;
+// split: split-TF32 operands (both split in-kernel)
+int conv_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st, bool split = false);
 // weight gradient of the style-modulated convolution (per-sample filters W * s[n]) from the unscaled input
 bool wgrad_modulated_eligible(const sae_conv_geom* g);
 int conv_wgrad_modulated(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
-                         const sae_conv_geom* g, cudaStream_t st);
+                         const sae_conv_geom* g, cudaStream_t st, bool split = false);
 
 // conv_wgmma.cu
 bool tc_available();
 bool tc_fprop_eligible(const sae_conv_geom* g);
 bool tc_dgrad_eligible(const sae_conv_geom* g);
-int tc_fprop(const float* x, const float* w, float* y, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st);
-int tc_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st);
+// w_lo / wt_lo non-null: split-TF32 operands, the filter given as the pair (w, w_lo) = (hi, lo) (sae_split_tf32)
+int tc_fprop(const float* x, const float* w, float* y, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st,
+             const float* w_lo = nullptr);
+int tc_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st,
+             const float* wt_lo = nullptr);
 // wgrad_wgmma.cu: weight gradient (plain and modulated) on wgmma; needs K % 4 == 0, C % 4 == 0, 16-byte aligned dy and x
 bool wgrad_wg_eligible(const sae_conv_geom* g);
-int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st);
+int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st,
+                    bool split = false);
 // style-modulated convolution: per-sample filters (forward / data gradient)
 bool tc_per_sample_eligible(const sae_conv_geom* g, int dgrad);
 int tc_conv_per_sample(const float* src, const float* w, float* out, const sae_conv_geom* g, int dgrad, const EpiParams& e,
-                       cudaStream_t st);
+                       cudaStream_t st, const float* w_lo = nullptr);
 
 }  // namespace sae

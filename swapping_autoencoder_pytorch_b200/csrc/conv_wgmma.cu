@@ -20,7 +20,8 @@
 // fprop uses it with taps (r - pad_t, s - pad_l); dgrad with taps (pad_t - r, pad_l - s) over dy and the [C, R*S*K]
 // transposed filter, a stride-2 data gradient as its four parity classes batched into one launch.  Operands are consumed
 // at TF32 precision (low 13 mantissa bits ignored by the tensor core); producers in this library round-to-nearest to TF32
-// so that this truncation is exact.
+// so that this truncation is exact.  The split-TF32 instantiations (SPLIT = true, the fp32 precision mode) take the filter
+// as a (hi, lo) pair of matrices, split the activation tile in registers and issue three register-A wgmma per k8 step.
 #include "tc_common.cuh"
 #include <mutex>
 
@@ -113,14 +114,20 @@ __device__ __forceinline__ void tc_epilogue_math(float (&v)[32], const EpiParams
     }
 }
 
-template <int BLOCK_N>
-constexpr int tc_stages() { return BLOCK_N >= 128 ? 3 : 4; }   // <= 96 KB of ring per CTA: two CTAs co-reside on an SM,
-                                                                // one runs its epilogue while the other feeds the tensor core
+// TF32: <= 96 KB of ring per CTA: two CTAs co-reside on an SM, one runs its epilogue while the other feeds the tensor core.
+// Split-TF32 (SPLIT: B_hi and B_lo tiles per stage, a second accumulator set): BLOCK_N = 64 and 32 only (at 128 the
+// accumulators, partial sums and split A fragments do not fit the registers without spills), 4 stages; BLOCK_N = 64 takes
+// 128 KB and its registers allow one CTA per SM, BLOCK_N = 32 keeps two (96 KB).
+template <int BLOCK_N, bool SPLIT>
+constexpr int tc_stages() { return SPLIT ? 4 : (BLOCK_N >= 128 ? 3 : 4); }
+template <int BLOCK_N, bool SPLIT>
+constexpr int tc_min_blocks() { return SPLIT && BLOCK_N >= 64 ? 1 : 2; }
 
-template <int BLOCK_N>
+template <int BLOCK_N, bool SPLIT>
 constexpr size_t tc_smem_bytes() {
-    // stage ring (A + B per stage); the epilogue staging (BLOCK_N/32 chunks of 16 KB) reuses it after the main loop.
-    size_t ring = (size_t)tc_stages<BLOCK_N>() * (TC_A_BYTES + BLOCK_N * 128);
+    // stage ring (A + B, or A + B_hi + B_lo, per stage); the epilogue staging (BLOCK_N/32 chunks of 16 KB) reuses it after the
+    // main loop.
+    size_t ring = (size_t)tc_stages<BLOCK_N, SPLIT>() * (TC_A_BYTES + (SPLIT ? 2 : 1) * BLOCK_N * 128);
     size_t epi = (size_t)(BLOCK_N / 32) * TC_A_BYTES;
     return (ring > epi ? ring : epi) + 1024 /*alignment slack*/ + 256 /*barriers*/;
 }
@@ -134,10 +141,18 @@ struct TcBatch {
     TcParams p[TC_MAX_BATCH];
     CUtensorMap src[TC_MAX_BATCH], out[TC_MAX_BATCH];
     CUtensorMap w;
+    CUtensorMap w_lo;                         // split-TF32 only: the low halves of the filter matrix, same geometry as w
 };
 
-template <int BLOCK_N>
-__global__ void __launch_bounds__(TC_THREADS, 2)
+// SPLIT = false: TF32 operands straight from shared memory (the default).  SPLIT = true: split-TF32, fp32-accurate products:
+// w arrives as the pair (hi, lo) = (rna_tf32(w), rna_tf32(w - hi)) in two filter matrices, the activation A is split in
+// registers, and every k8 step issues the register-A products A_hi B_hi + A_hi B_lo + A_lo B_hi (A_lo B_lo is below fp32
+// rounding and dropped).  The tensor core adds its products into the accumulator rounding toward zero; over thousands of
+// k8 steps that bias alone reaches ~1e-5 relative.  So the split path lets wgmma accumulate one stage (32 k) into the partial
+// sums `part` (the stage's first wgmma overwrites them: scale-d = 0) and adds `part` into `acc` with round-to-nearest fp32
+// adds once per stage.
+template <int BLOCK_N, bool SPLIT>
+__global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<BLOCK_N, SPLIT>())
 conv_wg_kernel(const __grid_constant__ TcBatch batch) {
     int prob = 0;
     while (prob + 1 < batch.count && (int)blockIdx.x >= batch.tile_end[prob]) ++prob;
@@ -145,9 +160,9 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
     const CUtensorMap& map_src = batch.src[prob];
     const CUtensorMap& map_out = batch.out[prob];
     const CUtensorMap& map_w = batch.w;
-    constexpr int STAGES = tc_stages<BLOCK_N>();
+    constexpr int STAGES = tc_stages<BLOCK_N, SPLIT>();
     constexpr int B_BYTES = BLOCK_N * 128;
-    constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
+    constexpr int STAGE_BYTES = TC_A_BYTES + (SPLIT ? 2 : 1) * B_BYTES;
     constexpr int NCHUNK = BLOCK_N / 32;
     constexpr int NACC = BLOCK_N / 2;                                   // fp32 accumulators per thread (m64 x BLOCK_N / 128)
 
@@ -175,6 +190,7 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_src) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
+        if constexpr (SPLIT) asm volatile("prefetch.tensormap [%0];" ::"l"(&batch.w_lo) : "memory");
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(bar_full + 8 * s, 1);
             mbar_init(bar_empty + 8 * s, TC_CONSUMERS / 32);          // one arrival per consumer warp
@@ -196,6 +212,7 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
                 mbar_expect_tx(bar_full + 8 * s, STAGE_BYTES);
                 tma_load_4d(sa, &map_src, bar_full + 8 * s, cb * TC_BK, q0 * p.stride + p.ox[t], p0 * p.stride + p.oy[t], n0);
                 tma_load_2d(sb, &map_w, bar_full + 8 * s, p.wk[t] + cb * TC_BK, wrow);
+                if constexpr (SPLIT) tma_load_2d(sb + B_BYTES, &batch.w_lo, bar_full + 8 * s, p.wk[t] + cb * TC_BK, wrow);
             }
         }
         return;
@@ -204,22 +221,58 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
     // ===================================================== consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64)
     const int wg = warp >> 2;
     float acc[NACC];
+    float part[SPLIT ? NACC : 1];                                      // split-TF32: the current stage's sums
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
     for (int kb = 0; kb < KB; ++kb) {
         const int s = kb % STAGES;
         mbar_wait(bar_full + 8 * s, (uint32_t)(kb / STAGES) & 1u);
         const uint32_t sa = base + (uint32_t)s * STAGE_BYTES, sb = sa + TC_A_BYTES;
-        const uint64_t da = make_wgmma_desc_sw128(sa + (uint32_t)wg * (64 * 128)), db = make_wgmma_desc_sw128(sb);
-        wgmma_fence();
+        if constexpr (SPLIT) {
+            // A fragments (m16 x k8 per warp, k steps k = 0..3) out of the swizzled stage: rows r = 64 wg + 16 (warp & 3) +
+            // lane / 4 (+ 8), columns 8 k + lane % 4 (+ 4).  r & 7 == lane / 4, so the 16-byte piece (2 k or 2 k + 1) ^ (lane / 4)
+            // and the word lane % 4 put the warp's 32 loads on 32 distinct banks.
+            const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+            const float* arow = reinterpret_cast<const float*>(smem_gen + (sa - base) + (uint32_t)r * 128) + (lane & 3);
+            uint32_t ahi[TC_BK / 8][4], alo[TC_BK / 8][4];
 #pragma unroll
-        for (int k = 0; k < TC_BK / 8; ++k) {
-            // advance 8 tf32 = 32 bytes along K inside the swizzle atom: +2 in the (addr >> 4) field
-            Wgmma<BLOCK_N>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
+            for (int k = 0; k < TC_BK / 8; ++k) {
+                const int p0 = ((2 * k) ^ (lane >> 2)) * 4, p1 = ((2 * k + 1) ^ (lane >> 2)) * 4;
+                split_tf32(arow[p0], ahi[k][0], alo[k][0]);
+                split_tf32(arow[8 * 32 + p0], ahi[k][1], alo[k][1]);
+                split_tf32(arow[p1], ahi[k][2], alo[k][2]);
+                split_tf32(arow[8 * 32 + p1], ahi[k][3], alo[k][3]);
+            }
+            const uint64_t db = make_wgmma_desc_sw128(sb), dbl = make_wgmma_desc_sw128(sb + B_BYTES);
+            wgmma_fence();
+            Wgmma<BLOCK_N>::template mma_rs<0>(part, alo[0], db);
+            Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[0], dbl);
+            Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[0], db);
+#pragma unroll
+            for (int k = 1; k < TC_BK / 8; ++k) {
+                Wgmma<BLOCK_N>::template mma_rs<1>(part, alo[k], db + (uint64_t)(k * 2));
+                Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[k], dbl + (uint64_t)(k * 2));
+                Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[k], db + (uint64_t)(k * 2));
+            }
+        } else {
+            const uint64_t da = make_wgmma_desc_sw128(sa + (uint32_t)wg * (64 * 128)), db = make_wgmma_desc_sw128(sb);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < TC_BK / 8; ++k) {
+                // advance 8 tf32 = 32 bytes along K inside the swizzle atom: +2 in the (addr >> 4) field
+                Wgmma<BLOCK_N>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
+            }
         }
         wgmma_commit();
-        wgmma_wait<1>();                                               // the group of stage kb - 1 has retired
-        if (kb > 0 && lane == 0) mbar_arrive(bar_empty + 8 * ((kb - 1) % STAGES));
+        if constexpr (SPLIT) {
+            wgmma_wait<0>();       // the next stage's A fragments reuse these registers: retire this group before loading them
+            if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+#pragma unroll
+            for (int i = 0; i < NACC; ++i) acc[i] += part[i];
+        } else {
+            wgmma_wait<1>();                                           // the group of stage kb - 1 has retired
+            if (kb > 0 && lane == 0) mbar_arrive(bar_empty + 8 * ((kb - 1) % STAGES));
+        }
     }
     wgmma_wait<0>();
 
@@ -286,6 +339,7 @@ int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims
 struct TcProblem {
     const float* src; int SN, SH, SW, SC;      // source activation [SN,SH,SW,SC]
     const float* wmat; int Ncol, Ktot;          // filter matrix [Ncol, Ktot = ntaps*SC]
+    const float* wmat_lo;                       // split-TF32: the low halves of wmat (same shape); nullptr = TF32 operands
     int w_per_sample;                           // 1: wmat holds one filter matrix per image, [SN, Ncol, Ktot]
     float* out; int OH, OW;                     // output sub-grid [SN, OH, OW, Ncol] ...
     int o_mul, o_offy, o_offx, FH, FW;          // ... placed at (o_mul*p + o_offy, o_mul*q + o_offx) of the full [SN,FH,FW,Ncol]
@@ -321,6 +375,14 @@ static void tc_fill_params(const TcProblem& pr, const EpiParams& e, TcParams& p)
     p.epi = e;
 }
 
+static int tc_encode_filter(const TcProblem& pr, const float* wmat, int b_rows, CUtensorMap* mw) {
+    cuuint64_t dims[2] = {(cuuint64_t)pr.Ktot, (cuuint64_t)pr.Ncol * (cuuint64_t)(pr.w_per_sample ? pr.SN : 1)};
+    cuuint64_t strides[1] = {(cuuint64_t)pr.Ktot * 4};
+    cuuint32_t box[2] = {32, (cuuint32_t)b_rows};
+    cuuint32_t es[2] = {1, 1};
+    return encode_map(mw, wmat, 2, dims, strides, box, es);
+}
+
 static int tc_encode_maps(const TcProblem& pr, const TcParams& p, int b_rows, CUtensorMap* msrc, CUtensorMap* mw, CUtensorMap* mout) {
     {
         cuuint64_t dims[4] = {(cuuint64_t)pr.SC, (cuuint64_t)pr.SW, (cuuint64_t)pr.SH, (cuuint64_t)pr.SN};
@@ -331,11 +393,7 @@ static int tc_encode_maps(const TcProblem& pr, const TcParams& p, int b_rows, CU
         if (rc) return rc;
     }
     {
-        cuuint64_t dims[2] = {(cuuint64_t)pr.Ktot, (cuuint64_t)pr.Ncol * (cuuint64_t)(pr.w_per_sample ? pr.SN : 1)};
-        cuuint64_t strides[1] = {(cuuint64_t)pr.Ktot * 4};
-        cuuint32_t box[2] = {32, (cuuint32_t)b_rows};
-        cuuint32_t es[2] = {1, 1};
-        int rc = encode_map(mw, pr.wmat, 2, dims, strides, box, es);
+        int rc = tc_encode_filter(pr, pr.wmat, b_rows, mw);
         if (rc) return rc;
     }
     {
@@ -351,7 +409,7 @@ static int tc_encode_maps(const TcProblem& pr, const TcParams& p, int b_rows, CU
 }
 
 // one-tile-per-CTA launch of up to TC_MAX_BATCH problems that share the filter matrix, the column count and the epilogue
-template <int BLOCK_N>
+template <int BLOCK_N, bool SPLIT>
 static int tc_launch_batch(const TcProblem* prs, int count, const EpiParams& e, cudaStream_t st) {
     TcBatch b;
     if (count < 1 || count > TC_MAX_BATCH) return fail(SAE_E_INVALID, "conv_wg: batch of %d problems", count);
@@ -364,31 +422,41 @@ static int tc_launch_batch(const TcProblem* prs, int count, const EpiParams& e, 
         int rc = tc_encode_maps(prs[i], b.p[i], BLOCK_N, &b.src[i], &mw, &b.out[i]);
         if (rc) return rc;
         if (i == 0) b.w = mw;
-        else if (prs[i].wmat != prs[0].wmat || prs[i].Ncol != prs[0].Ncol || prs[i].Ktot != prs[0].Ktot)
+        else if (prs[i].wmat != prs[0].wmat || prs[i].wmat_lo != prs[0].wmat_lo || prs[i].Ncol != prs[0].Ncol ||
+                 prs[i].Ktot != prs[0].Ktot)
             return fail(SAE_E_INVALID, "conv_wg: batched problems must share the filter matrix");
         tiles += b.p[i].tiles_w * b.p[i].tiles_h * b.p[i].tiles_n;
         b.tile_end[i] = tiles;
     }
-    constexpr size_t smem = tc_smem_bytes<BLOCK_N>();
+    if (SPLIT) {
+        int rc = tc_encode_filter(prs[0], prs[0].wmat_lo, BLOCK_N, &b.w_lo);
+        if (rc) return rc;
+    }
+    constexpr size_t smem = tc_smem_bytes<BLOCK_N, SPLIT>();
     static bool attr_done = false;
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_wg_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_wg_kernel<BLOCK_N, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done = true;
     }
     dim3 grid((unsigned)tiles, (unsigned)(prs[0].Ncol / BLOCK_N));
-    conv_wg_kernel<BLOCK_N><<<grid, TC_THREADS, smem, st>>>(b);
+    conv_wg_kernel<BLOCK_N, SPLIT><<<grid, TC_THREADS, smem, st>>>(b);
     return check_launch("conv_wg");
 }
 
 static int tc_dispatch(const TcProblem* prs, int count, const EpiParams& e, cudaStream_t st) {
     const int ncol = prs[0].Ncol;
-    if (ncol % 128 == 0) return tc_launch_batch<128>(prs, count, e, st);
-    if (ncol % 64 == 0) return tc_launch_batch<64>(prs, count, e, st);
-    return tc_launch_batch<32>(prs, count, e, st);
+    if (prs[0].wmat_lo) {
+        if (ncol % 64 == 0) return tc_launch_batch<64, true>(prs, count, e, st);
+        return tc_launch_batch<32, true>(prs, count, e, st);
+    }
+    if (ncol % 128 == 0) return tc_launch_batch<128, false>(prs, count, e, st);
+    if (ncol % 64 == 0) return tc_launch_batch<64, false>(prs, count, e, st);
+    return tc_launch_batch<32, false>(prs, count, e, st);
 }
 
-static bool ptr_ok(const void* a, const void* b, const void* c) {
-    return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
+static bool ptr_ok(const void* a, const void* b, const void* c, const void* d = nullptr) {
+    return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
+             reinterpret_cast<uintptr_t>(d)) & 15) == 0;
 }
 
 bool tc_fprop_eligible(const sae_conv_geom* g) {
@@ -404,10 +472,12 @@ bool tc_dgrad_eligible(const sae_conv_geom* g) {
     return tc_shape_ok(g->K, g->C, g->R * g->S, 1, (g->W + g->stride - 1) / g->stride);
 }
 
-int tc_fprop(const float* x, const float* w, float* y, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st) {
-    if (!ptr_ok(x, w, y)) return fail(SAE_E_INVALID, "conv2d_fprop(wgmma): pointers must be 16-byte aligned");
+int tc_fprop(const float* x, const float* w, float* y, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st,
+             const float* w_lo) {
+    if (!ptr_ok(x, w, y, w_lo)) return fail(SAE_E_INVALID, "conv2d_fprop(wgmma): pointers must be 16-byte aligned");
     TcProblem pr;
     pr.w_per_sample = 0;
+    pr.wmat_lo = w_lo;
     pr.src = x; pr.SN = g->N; pr.SH = g->H; pr.SW = g->W; pr.SC = g->C;
     pr.wmat = w; pr.Ncol = g->K; pr.Ktot = g->R * g->S * g->C;
     pr.out = y; pr.OH = g->P; pr.OW = g->Q;
@@ -433,11 +503,13 @@ bool tc_per_sample_eligible(const sae_conv_geom* g, int dgrad) {
     return (int64_t)g->N * oh * ow >= 2 * 128;
 }
 
-int tc_conv_per_sample(const float* src, const float* w, float* out, const sae_conv_geom* g, int dgrad, const EpiParams& e, cudaStream_t st) {
+int tc_conv_per_sample(const float* src, const float* w, float* out, const sae_conv_geom* g, int dgrad, const EpiParams& e, cudaStream_t st,
+                       const float* w_lo) {
     if (!tc_per_sample_eligible(g, dgrad)) return fail(SAE_E_UNSUPPORTED, "per-sample conv: shape outside the per-sample kernel");
-    if (!ptr_ok(src, w, out)) return fail(SAE_E_INVALID, "per-sample conv: pointers must be 16-byte aligned");
+    if (!ptr_ok(src, w, out, w_lo)) return fail(SAE_E_INVALID, "per-sample conv: pointers must be 16-byte aligned");
     TcProblem pr;
     pr.w_per_sample = 1;
+    pr.wmat_lo = w_lo;
     pr.stride = 1; pr.o_mul = 1; pr.o_offy = 0; pr.o_offx = 0; pr.ntaps = g->R * g->S;
     pr.src = src; pr.wmat = w; pr.out = out; pr.SN = g->N;
     if (!dgrad) {
@@ -457,10 +529,12 @@ int tc_conv_per_sample(const float* src, const float* w, float* out, const sae_c
     return tc_dispatch(&pr, 1, e, st);
 }
 
-int tc_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st) {
-    if (!ptr_ok(dy, wt, dx)) return fail(SAE_E_INVALID, "conv2d_dgrad(wgmma): pointers must be 16-byte aligned");
+int tc_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st,
+             const float* wt_lo) {
+    if (!ptr_ok(dy, wt, dx, wt_lo)) return fail(SAE_E_INVALID, "conv2d_dgrad(wgmma): pointers must be 16-byte aligned");
     TcProblem pr;
     pr.w_per_sample = 0;
+    pr.wmat_lo = wt_lo;
     pr.src = dy; pr.SN = g->N; pr.SH = g->P; pr.SW = g->Q; pr.SC = g->K;
     pr.wmat = wt; pr.Ncol = g->C; pr.Ktot = g->R * g->S * g->K;
     pr.stride = 1; pr.FH = g->H; pr.FW = g->W;

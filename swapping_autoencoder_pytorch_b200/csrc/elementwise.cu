@@ -707,6 +707,23 @@ extern "C" int sae_round_tf32(const float* x, float* out, int64_t n, void* strea
     return sae_add_scale(x, nullptr, out, n, 1.0f, 1, stream);
 }
 
+// filter pair of the split-TF32 convolutions: hi = rna_tf32(x), lo = rna_tf32(x - hi)
+__global__ void split_tf32_kernel(const float* __restrict__ x, float* __restrict__ hi, float* __restrict__ lo, int64_t n) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        uint32_t h, l;
+        split_tf32(__ldg(x + i), h, l);
+        hi[i] = __uint_as_float(h);
+        lo[i] = __uint_as_float(l);
+    }
+}
+
+extern "C" int sae_split_tf32(const float* x, float* hi, float* lo, int64_t n, void* stream) {
+    if (n == 0) return SAE_OK;
+    if (!x || !hi || !lo || n < 0) return fail(SAE_E_INVALID, "split_tf32: bad arguments");
+    split_tf32_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(x, hi, lo, n);
+    return check_launch("split_tf32");
+}
+
 extern "C" int sae_bucket_pack(const float* const* ptrs, const int64_t* offsets, const int64_t* sizes, int n,
                                float* bucket, int64_t total, void* stream) {
     if (n == 0) return SAE_OK;

@@ -112,7 +112,9 @@ __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uin
 }
 
 // D[64 x 128] += A[64 x 8] * B[128 x 8]^T with A from registers (tf32 bits; per warp the m16n8k8 A fragment: rows lane / 4
-// (+ 8 for a1 / a3), columns lane % 4 (+ 4 for a2 / a3)), B from shared memory through its descriptor
+// (+ 8 for a1 / a3), columns lane % 4 (+ 4 for a2 / a3)), B from shared memory through its descriptor.  SCALE_D = 0: D = A B
+// (the previous contents of d are ignored)
+template <int SCALE_D = 1>
 __device__ __forceinline__ void wgmma_tf32_n128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
     asm volatile("wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
                  "{"
@@ -120,7 +122,7 @@ __device__ __forceinline__ void wgmma_tf32_n128_rs(float (&d)[64], const uint32_
                  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
                  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
                  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-                 "}, {%64, %65, %66, %67}, %68, 1, 1, 1;"
+                 "}, {%64, %65, %66, %67}, %68, %69, 1, 1;"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
                    "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
                    "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
@@ -129,12 +131,49 @@ __device__ __forceinline__ void wgmma_tf32_n128_rs(float (&d)[64], const uint32_
                    "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
                    "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
                    "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(SCALE_D));
+}
+
+// the n32 / n64 register-A forms (split-TF32 mode of conv_wgmma.cu), same A fragment layout as wgmma_tf32_n128_rs
+template <int SCALE_D = 1>
+__device__ __forceinline__ void wgmma_tf32_n32_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+                 "{"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+                 "}, {%16, %17, %18, %19}, %20, %21, 1, 1;"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(SCALE_D));
+}
+template <int SCALE_D = 1>
+__device__ __forceinline__ void wgmma_tf32_n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile("wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+                 "{"
+                 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+                 "}, {%32, %33, %34, %35}, %36, %37, 1, 1;"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "n"(SCALE_D));
 }
 
 template <int N> struct Wgmma;
-template <> struct Wgmma<32> { static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b) { wgmma_tf32_n32(d, a, b); } };
-template <> struct Wgmma<64> { static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b) { wgmma_tf32_n64(d, a, b); } };
-template <> struct Wgmma<128> { static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b) { wgmma_tf32_n128(d, a, b); } };
+template <> struct Wgmma<32> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b) { wgmma_tf32_n32(d, a, b); }
+    template <int SCALE_D>
+    static __device__ __forceinline__ void mma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b) { wgmma_tf32_n32_rs<SCALE_D>(d, a, b); }
+};
+template <> struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b) { wgmma_tf32_n64(d, a, b); }
+    template <int SCALE_D>
+    static __device__ __forceinline__ void mma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b) { wgmma_tf32_n64_rs<SCALE_D>(d, a, b); }
+};
+template <> struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b) { wgmma_tf32_n128(d, a, b); }
+    template <int SCALE_D>
+    static __device__ __forceinline__ void mma_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b) { wgmma_tf32_n128_rs<SCALE_D>(d, a, b); }
+};
 
 }  // namespace sae

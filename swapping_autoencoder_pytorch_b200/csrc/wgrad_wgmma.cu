@@ -17,6 +17,11 @@
 //     forms dW += s[n, c] G_n and ds[n, c] += sum_{o, tap} W[o, tap, c] G_n from the unscaled input (ds summed over the
 //     CTA's 128 rows in shared memory, one atomic per column).
 // Operands are rounded to TF32 (cvt.rna) on their way into the fragments / the transposed tile, as in the mma.sync kernel.
+// Split-TF32 (SPLIT = true, the fp32 precision mode): every operand is split into hi = rna_tf32(v), lo = rna_tf32(v - hi); the
+// dy fragments in registers, the gathered x into a hi and a lo K-major tile (+16 KB), and each k8 step issues
+// dy_lo x_hi + dy_hi x_lo + dy_hi x_hi.  The tensor core's accumulation rounds toward zero, so these wgmma accumulate one stage
+// into partial sums (scale-d = 0 on the first) that are added into the accumulators with round-to-nearest fp32 adds; with the
+// second accumulator set the kernel runs one CTA per SM.
 #include "tc_common.cuh"
 
 namespace sae {
@@ -26,21 +31,24 @@ constexpr int WGR_BK = 32;                        // pixels per stage
 constexpr int WGR_LD = 128 + 8;                   // row stride (floats) of the pixel-major staging tiles
 constexpr int WGR_TILE = WGR_BK * WGR_LD * 4;     // bytes of one pixel-major tile
 constexpr int WGR_BT = 128 * WGR_BK * 4;          // the K-major swizzled B tile: 128 rows x 128 bytes = 16 KB
-constexpr size_t WGR_SMEM = (size_t)WGR_BT + 4 * (size_t)WGR_TILE + 1024;
+template <bool SPLIT>
+constexpr size_t wgr_smem() { return (size_t)(SPLIT ? 2 : 1) * WGR_BT + 4 * (size_t)WGR_TILE + 1024; }
 
 __device__ __forceinline__ void cp_async16_wg(uint32_t s, const void* gmem, bool pred) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(pred ? 16 : 0));
 }
 
-__global__ void __launch_bounds__(WGR_THREADS, 2)
+template <bool SPLIT>
+__global__ void __launch_bounds__(WGR_THREADS, SPLIT ? 1 : 2)
 wgrad_wg_kernel(const float* __restrict__ dy, const float* __restrict__ x, float* __restrict__ dw, const WgradParams p) {
+    constexpr int BT_BYTES = (SPLIT ? 2 : 1) * WGR_BT;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-byte alignment
     uint8_t* smem_gen = smem_raw + (base - smem_u32(smem_raw));
-    uint8_t* bt = smem_gen;                                            // K-major B tile
+    uint8_t* bt = smem_gen;                                            // K-major B tile (SPLIT: hi, then lo)
     const uint32_t bt_s = base;
-    float* tiles = reinterpret_cast<float*>(smem_gen + WGR_BT);        // [stage][A, B][WGR_BK][WGR_LD]
-    const uint32_t tiles_s = base + WGR_BT;
+    float* tiles = reinterpret_cast<float*>(smem_gen + BT_BYTES);      // [stage][A, B][WGR_BK][WGR_LD]
+    const uint32_t tiles_s = base + BT_BYTES;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
     const int g = lane >> 2, t = lane & 3;
@@ -81,6 +89,7 @@ wgrad_wg_kernel(const float* __restrict__ dy, const float* __restrict__ x, float
     };
 
     float acc[64];
+    float part[SPLIT ? 64 : 1];                                        // split-TF32: the current stage's sums
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     if (KB > 0) load_stage(0, 0);
@@ -93,36 +102,77 @@ wgrad_wg_kernel(const float* __restrict__ dy, const float* __restrict__ x, float
         asm volatile("cp.async.commit_group;" ::: "memory");
         const float* at = tiles + (size_t)(2 * (kb & 1)) * (WGR_TILE / 4);
         const float* bsrc = at + WGR_TILE / 4;
-        // B: pixel-major [32][136] -> K-major swizzled [128 rows][32 pixels]
+        if constexpr (SPLIT) {
+            // B_hi, B_lo: the same transpose, two tiles
 #pragma unroll
-        for (int qd = 0; qd < 4; ++qd) {
-            const int idx = tid + WGR_THREADS * qd;
-            const int n = idx & 127, c4 = idx >> 7;                    // column n, pixels 4 c4 .. 4 c4 + 3
-            float4 v;
-            v.x = rna_tf32(bsrc[(4 * c4 + 0) * WGR_LD + n]);
-            v.y = rna_tf32(bsrc[(4 * c4 + 1) * WGR_LD + n]);
-            v.z = rna_tf32(bsrc[(4 * c4 + 2) * WGR_LD + n]);
-            v.w = rna_tf32(bsrc[(4 * c4 + 3) * WGR_LD + n]);
-            *reinterpret_cast<float4*>(bt + n * 128 + ((c4 ^ (n & 7)) << 4)) = v;
+            for (int qd = 0; qd < 4; ++qd) {
+                const int idx = tid + WGR_THREADS * qd;
+                const int n = idx & 127, c4 = idx >> 7;
+                uint32_t h[4], l[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) split_tf32(bsrc[(4 * c4 + u) * WGR_LD + n], h[u], l[u]);
+                const int off = n * 128 + ((c4 ^ (n & 7)) << 4);
+                *reinterpret_cast<uint4*>(bt + off) = make_uint4(h[0], h[1], h[2], h[3]);
+                *reinterpret_cast<uint4*>(bt + WGR_BT + off) = make_uint4(l[0], l[1], l[2], l[3]);
+            }
+            uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+                const float* ap = at + (ks * 8 + t) * WGR_LD + r0;
+                split_tf32(ap[0], ahi[ks][0], alo[ks][0]);
+                split_tf32(ap[8], ahi[ks][1], alo[ks][1]);
+                split_tf32(ap[4 * WGR_LD], ahi[ks][2], alo[ks][2]);
+                split_tf32(ap[4 * WGR_LD + 8], ahi[ks][3], alo[ks][3]);
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncthreads();
+            const uint64_t db = make_wgmma_desc_sw128(bt_s), dbl = make_wgmma_desc_sw128(bt_s + WGR_BT);
+            wgmma_fence();
+            wgmma_tf32_n128_rs<0>(part, alo[0], db);
+            wgmma_tf32_n128_rs<1>(part, ahi[0], dbl);
+            wgmma_tf32_n128_rs<1>(part, ahi[0], db);
+#pragma unroll
+            for (int ks = 1; ks < 4; ++ks) {
+                wgmma_tf32_n128_rs<1>(part, alo[ks], db + (uint64_t)(ks * 2));
+                wgmma_tf32_n128_rs<1>(part, ahi[ks], dbl + (uint64_t)(ks * 2));
+                wgmma_tf32_n128_rs<1>(part, ahi[ks], db + (uint64_t)(ks * 2));
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] += part[i];
+        } else {
+            // B: pixel-major [32][136] -> K-major swizzled [128 rows][32 pixels]
+#pragma unroll
+            for (int qd = 0; qd < 4; ++qd) {
+                const int idx = tid + WGR_THREADS * qd;
+                const int n = idx & 127, c4 = idx >> 7;                    // column n, pixels 4 c4 .. 4 c4 + 3
+                float4 v;
+                v.x = rna_tf32(bsrc[(4 * c4 + 0) * WGR_LD + n]);
+                v.y = rna_tf32(bsrc[(4 * c4 + 1) * WGR_LD + n]);
+                v.z = rna_tf32(bsrc[(4 * c4 + 2) * WGR_LD + n]);
+                v.w = rna_tf32(bsrc[(4 * c4 + 3) * WGR_LD + n]);
+                *reinterpret_cast<float4*>(bt + n * 128 + ((c4 ^ (n & 7)) << 4)) = v;
+            }
+            // A: m16 x k8 fragments of dy^T (rows = out channels, columns = pixels) from the pixel-major tile
+            uint32_t a[4][4];
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+                const float* ap = at + (ks * 8 + t) * WGR_LD + r0;
+                a[ks][0] = __float_as_uint(rna_tf32(ap[0]));
+                a[ks][1] = __float_as_uint(rna_tf32(ap[8]));
+                a[ks][2] = __float_as_uint(rna_tf32(ap[4 * WGR_LD]));
+                a[ks][3] = __float_as_uint(rna_tf32(ap[4 * WGR_LD + 8]));
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy stores -> visible to wgmma
+            __syncthreads();
+            const uint64_t db = make_wgmma_desc_sw128(bt_s);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) wgmma_tf32_n128_rs(acc, a[ks], db + (uint64_t)(ks * 2));   // +32 bytes along K
+            wgmma_commit();
+            wgmma_wait<0>();
         }
-        // A: m16 x k8 fragments of dy^T (rows = out channels, columns = pixels) from the pixel-major tile
-        uint32_t a[4][4];
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-            const float* ap = at + (ks * 8 + t) * WGR_LD + r0;
-            a[ks][0] = __float_as_uint(rna_tf32(ap[0]));
-            a[ks][1] = __float_as_uint(rna_tf32(ap[8]));
-            a[ks][2] = __float_as_uint(rna_tf32(ap[4 * WGR_LD]));
-            a[ks][3] = __float_as_uint(rna_tf32(ap[4 * WGR_LD + 8]));
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");    // generic-proxy stores -> visible to wgmma
-        __syncthreads();
-        const uint64_t db = make_wgmma_desc_sw128(bt_s);
-        wgmma_fence();
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) wgmma_tf32_n128_rs(acc, a[ks], db + (uint64_t)(ks * 2));   // +32 bytes along K
-        wgmma_commit();
-        wgmma_wait<0>();
     }
 
     // accumulator fragment: rows o0 + r0 (+ 8), columns n0 + 8 j + 2 t + {0, 1}
@@ -179,15 +229,21 @@ wgrad_wg_kernel(const float* __restrict__ dy, const float* __restrict__ x, float
 
 bool wgrad_wg_eligible(const sae_conv_geom* g) { return g->K % 4 == 0 && g->C % 4 == 0; }
 
-int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st) {
+template <bool SPLIT>
+static int wgrad_wg_launch_t(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st) {
+    constexpr size_t smem = wgr_smem<SPLIT>();
     static bool attr_done = false;
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(wgrad_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WGR_SMEM));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(wgrad_wg_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done = true;
     }
     dim3 grid((unsigned)((p.Ko + 127) / 128), (unsigned)((p.Ncol + 127) / 128), splits);
-    wgrad_wg_kernel<<<grid, WGR_THREADS, WGR_SMEM, st>>>(dy, x, dw, p);
+    wgrad_wg_kernel<SPLIT><<<grid, WGR_THREADS, smem, st>>>(dy, x, dw, p);
     return check_launch("wgrad_wg");
+}
+
+int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st, bool split) {
+    return split ? wgrad_wg_launch_t<true>(dy, x, dw, p, splits, st) : wgrad_wg_launch_t<false>(dy, x, dw, p, splits, st);
 }
 
 }  // namespace sae

@@ -22,7 +22,7 @@ import warnings
 
 import torch
 
-from . import _lib
+from . import _lib, backend
 
 
 class HalfStepGraphs:
@@ -30,7 +30,7 @@ class HalfStepGraphs:
         self.trainer = trainer
         self.warmup = warmup
         self.calls = {}
-        self.captured = {}        # kind -> (graph, static_input, static_outputs, launches)
+        self.captured = {}        # (kind, input shape, kernel precision) -> (graph, static_input, static_outputs, launches)
         self.pool = None
         self.stream = None             # side stream shared by the eager warm-up calls and every capture (see _side)
         self.disabled = None
@@ -96,9 +96,12 @@ class HalfStepGraphs:
     def run(self, kind, body, images):
         if self.disabled is not None or not self.enabled:
             return body(images)
-        n = self.calls.get(kind, 0)
-        self.calls[kind] = n + 1
-        key = (kind, tuple(images.shape))
+        # a graph records the kernels of one precision mode (backend.CudaKernels.precision): switching the mode captures new
+        # graphs, after warm-up calls of their own (the other mode's kernels initialise lazily, outside any capture)
+        precision = getattr(backend.kernels(), "precision", "tf32")
+        n = self.calls.get((kind, precision), 0)
+        self.calls[(kind, precision)] = n + 1
+        key = (kind, tuple(images.shape), precision)
         hit = self.captured.get(key)
         if hit is None:
             if n < self.warmup:

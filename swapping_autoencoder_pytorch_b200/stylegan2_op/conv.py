@@ -107,11 +107,13 @@ def filter_reuse():
 
 
 def memo(source, tag, build):
-    """``build()`` once per (source tensor identity and version, tag, grad mode) inside ``filter_reuse()``; outside a scope it
-    is always rebuilt.  The entry keeps ``source`` alive so its id cannot be recycled while the scope is open."""
+    """``build()`` once per (source tensor identity and version, tag, grad mode, kernel precision) inside ``filter_reuse()``;
+    outside a scope it is always rebuilt.  The precision is part of the key because the prepared filters differ between the
+    modes (TF32-rounded or not).  The entry keeps ``source`` alive so its id cannot be recycled while the scope is open."""
     if _FilterMemo.depth == 0:
         return build()
-    key = (id(source), source._version, tag, torch.is_grad_enabled(), source.requires_grad)
+    key = (id(source), source._version, tag, torch.is_grad_enabled(), source.requires_grad,
+           getattr(backend.kernels(), "precision", "tf32"))
     hit = _FilterMemo.store.get(key)
     if hit is None:
         hit = (source, build())
