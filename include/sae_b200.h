@@ -228,7 +228,7 @@ int sae_conv2d_fprop(const float* x, const float* w, float* y, const sae_conv_ge
 int sae_conv2d_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g,
                      const sae_conv_epilogue* epi, int impl, void* stream);
 /* dw [K,R,S,C] is ACCUMULATED into (split-K reduction with fp32 atomics): zero it first.  impl as above; the wgmma kernel
- * takes K % 4 == 0, C % 4 == 0 and 16-byte aligned dy / x. */
+ * takes K % 32 == 0, C % 32 == 0, stride 1 or 2 and 16-byte aligned dy / x. */
 int sae_conv2d_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g,
                      int impl, void* stream);
 

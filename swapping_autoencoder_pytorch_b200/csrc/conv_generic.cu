@@ -621,6 +621,9 @@ static int wgrad_impl(const float* dy, const float* x, float* dw, const sae_conv
     p.Ncol = g->R * g->S * g->C;
     p.Mpix = (int64_t)g->N * g->P * g->Q;
     if (p.Mpix == 0 || p.Ko == 0 || p.Ncol == 0) return SAE_OK;
+    const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) == 0;
+    const bool wg_ok = impl != 1 && al && wgrad_wg_eligible(g) && tc_available();
+    if (wg_ok && !split) return wgrad_wg_launch(dy, x, dw, p, st);
     int64_t tiles = (int64_t)((p.Ko + 127) / 128) * ((p.Ncol + 127) / 128);
     int64_t want = ((int64_t)sm_count() * 2 + tiles - 1) / tiles;      // ~2 CTAs per SM
     int64_t kblocks = (p.Mpix + BK - 1) / BK;
@@ -632,9 +635,8 @@ static int wgrad_impl(const float* dy, const float* x, float* dw, const sae_conv
         while ((p.img_pix / BK) % kb_per != 0) --kb_per;      // chunks must not straddle images (img_pix % BK == 0)
     p.chunk = kb_per * BK;
     unsigned splits = (unsigned)((p.Mpix + p.chunk - 1) / p.chunk);
-    const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) == 0;
     const bool va = (p.Ko % 4 == 0) && al, vb = (p.C % 4 == 0) && al;
-    if (impl != 1 && va && vb && tc_available()) return wgrad_wg_launch(dy, x, dw, p, splits, st, split);
+    if (wg_ok) return wgrad_split_launch(dy, x, dw, p, splits, st);
     return split ? launch_wgrad_any<true>(dy, x, dw, p, splits, st, va, vb) : launch_wgrad_any<false>(dy, x, dw, p, splits, st, va, vb);
 }
 

@@ -52,10 +52,12 @@ int tc_fprop(const float* x, const float* w, float* y, const sae_conv_geom* g, c
              const float* w_lo = nullptr);
 int tc_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st,
              const float* wt_lo = nullptr);
-// wgrad_wgmma.cu: weight gradient (plain and modulated) on wgmma; needs K % 4 == 0, C % 4 == 0, 16-byte aligned dy and x
+// wgrad_wgmma.cu: weight gradient (plain and modulated) on wgmma; needs K % 32 == 0, C % 32 == 0, stride 1 or 2, and
+// 16-byte aligned dy and x (other shapes take the mma.sync kernel).  wgrad_wg_launch: TF32 operands, TMA-fed pipeline,
+// chooses its own pixel splits; wgrad_split_launch: split-TF32 operands, p.chunk pixels per split
 bool wgrad_wg_eligible(const sae_conv_geom* g);
-int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st,
-                    bool split = false);
+int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& p, cudaStream_t st);
+int wgrad_split_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st);
 // style-modulated convolution: per-sample filters (forward / data gradient)
 bool tc_per_sample_eligible(const sae_conv_geom* g, int dgrad);
 int tc_conv_per_sample(const float* src, const float* w, float* out, const sae_conv_geom* g, int dgrad, const EpiParams& e,

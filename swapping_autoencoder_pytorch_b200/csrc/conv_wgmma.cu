@@ -360,11 +360,7 @@ static void tc_fill_params(const TcProblem& pr, const EpiParams& e, TcParams& p)
     p.num_cblk = pr.SC / 32;
     p.ntaps = pr.ntaps;
     p.stride = pr.stride;
-    p.tw = pow2_ceil(pr.OW) < 16 ? pow2_ceil(pr.OW) : 16;
-    int th = 128 / p.tw;
-    if (pow2_ceil(pr.OH) < th) th = pow2_ceil(pr.OH);
-    p.th = th;
-    p.tn = 128 / (p.tw * p.th);
+    tile_box(pr.OH, pr.OW, 128, 16, p.tw, p.th, p.tn);
     p.tiles_w = (pr.OW + p.tw - 1) / p.tw;
     p.tiles_h = (pr.OH + p.th - 1) / p.th;
     p.tiles_n = (pr.SN + p.tn - 1) / p.tn;
@@ -383,13 +379,17 @@ static int tc_encode_filter(const TcProblem& pr, const float* wmat, int b_rows, 
     return encode_map(mw, wmat, 2, dims, strides, box, es);
 }
 
+int encode_act_map(CUtensorMap* m, const float* ptr, int N, int H, int W, int C, int tw, int th, int tn, int stride) {
+    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+    cuuint64_t strides[3] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
+    cuuint32_t box[4] = {32, (cuuint32_t)(tw * stride), (cuuint32_t)(th * stride), (cuuint32_t)tn};
+    cuuint32_t es[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+    return encode_map(m, ptr, 4, dims, strides, box, es);
+}
+
 static int tc_encode_maps(const TcProblem& pr, const TcParams& p, int b_rows, CUtensorMap* msrc, CUtensorMap* mw, CUtensorMap* mout) {
     {
-        cuuint64_t dims[4] = {(cuuint64_t)pr.SC, (cuuint64_t)pr.SW, (cuuint64_t)pr.SH, (cuuint64_t)pr.SN};
-        cuuint64_t strides[3] = {(cuuint64_t)pr.SC * 4, (cuuint64_t)pr.SW * pr.SC * 4, (cuuint64_t)pr.SH * pr.SW * pr.SC * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)(p.tw * pr.stride), (cuuint32_t)(p.th * pr.stride), (cuuint32_t)p.tn};
-        cuuint32_t es[4] = {1, (cuuint32_t)pr.stride, (cuuint32_t)pr.stride, 1};
-        int rc = encode_map(msrc, pr.src, 4, dims, strides, box, es);
+        int rc = encode_act_map(msrc, pr.src, pr.SN, pr.SH, pr.SW, pr.SC, p.tw, p.th, p.tn, pr.stride);
         if (rc) return rc;
     }
     {

@@ -18,6 +18,19 @@ inline int pow2_ceil(int v) {
     return p;
 }
 
+// Pixel box of a conv tile: tw x th x tn = `pixels` (a power of two) output pixels of an [N, OH, OW] grid, widest first,
+// tw <= tw_max.  Ragged edges are left to the TMA unit's zero fill (loads) and clipping (stores).
+inline void tile_box(int OH, int OW, int pixels, int tw_max, int& tw, int& th, int& tn) {
+    tw = pow2_ceil(OW) < tw_max ? pow2_ceil(OW) : tw_max;
+    th = pixels / tw;
+    if (pow2_ceil(OH) < th) th = pow2_ceil(OH);
+    tn = pixels / (tw * th);
+}
+
+// 4-D tensor map of an NHWC activation [N, H, W, C] whose box is 32 channels x (tw x th x tn) pixels taken every `stride`
+// pixels (a strided conv's input as seen from a box of its output), landing in the K-major 128-byte swizzle.
+int encode_act_map(CUtensorMap* m, const float* ptr, int N, int H, int W, int C, int tw, int th, int tn, int stride);
+
 // ------------------------------------------------------------------------------------------------ device helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
