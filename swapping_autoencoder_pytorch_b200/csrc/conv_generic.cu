@@ -253,7 +253,7 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
     }
     cp_async_wait<0>();
 
-    // epilogue
+    // epilogue (split-K runs only with the plain epilogue; launch_gather applies round_tf32 to the summed output)
     if (split) {
 #pragma unroll
         for (int i = 0; i < MT; ++i)
@@ -568,7 +568,10 @@ static int launch_gather(const float* src, const float* wmat, float* out, const 
         }
     }
     conv_gather_kernel<BN, VEC, SPLIT><<<grid, NTHREADS, smem, st>>>(src, wmat, out, p, e, wlo);
-    return check_launch("conv_gather");
+    int rc = check_launch("conv_gather");
+    // the split-K CTAs add raw partial sums into out: round the finished sums once they are all in
+    if (rc == SAE_OK && grid.z > 1 && e.round_tf32) rc = sae_round_tf32(out, out, p.M * p.Ncol, st);
+    return rc;
 }
 
 template <bool SPLIT>

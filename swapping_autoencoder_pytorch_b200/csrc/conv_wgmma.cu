@@ -529,6 +529,29 @@ int tc_conv_per_sample(const float* src, const float* w, float* out, const sae_c
     return tc_dispatch(&pr, 1, e, st);
 }
 
+// The pixels of the stride-2 parity classes that no filter tap reaches (bit 2 (y & 1) + (x & 1) of `empty`): the epilogue of
+// a zero accumulator, in the order of tc_epilogue_math, and their activation mask words.  One thread per element of dx; with
+// C % 32 == 0 (the wgmma path's column granularity) the 32 lanes of a warp are the 32 channels of one pixel = one mask word.
+__global__ void __launch_bounds__(256)
+tc_dgrad_empty_kernel(float* __restrict__ dx, const EpiParams e, int64_t total, int H, int W, int C, unsigned empty) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t pixel = i / C;
+        const int col = (int)(i - pixel * C);
+        const int x = (int)(pixel % W), y = (int)((pixel / W) % H);
+        if (!((empty >> ((y & 1) * 2 + (x & 1))) & 1u)) continue;        // uniform over the warp
+        float t = 0.f;
+        if (e.bias) t += __ldg(e.bias + col);
+        if (e.noise) t += __ldg(e.noise_weight) * __ldg(e.noise + pixel);
+        const uint32_t pos = __ballot_sync(0xffffffffu, t > 0.f);
+        if (e.act == 3) t = t > 0.f ? t : t * e.alpha;
+        t *= e.gain;
+        if (e.act_mask && (i & 31) == 0) e.act_mask[i >> 5] = pos;
+        if (e.residual) t = (t + __ldg(e.residual + i)) * e.res_scale;
+        if (e.round_tf32) t = rna_tf32(t);
+        dx[i] = t;
+    }
+}
+
 int tc_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g, const EpiParams& e, cudaStream_t st,
              const float* wt_lo) {
     if (!ptr_ok(dy, wt, dx, wt_lo)) return fail(SAE_E_INVALID, "conv2d_dgrad(wgmma): pointers must be 16-byte aligned");
@@ -553,13 +576,26 @@ int tc_dgrad(const float* dy, const float* wt, float* dx, const sae_conv_geom* g
     // splits into 4 parity classes (ho, wo); class outputs x[2i+ho, 2j+wo] only see taps with r = (ho + pad_t) mod 2,
     // s = (wo + pad_l) mod 2, read at source offset (ho + pad_t - r) / 2 — four dense stride-1 problems writing
     // interleaved sub-grids (the output tensor map carries the doubled strides), batched into one launch.
-    bool need_zero = false;
+    // a class no tap reaches (R == 1 or S == 1) has a zero accumulator: with a trivial epilogue its pixels are 0, otherwise
+    // they take the epilogue of 0 and their mask words from tc_dgrad_empty_kernel
+    unsigned empty = 0;
     for (int ho = 0; ho < 2; ++ho)
         for (int wo = 0; wo < 2; ++wo) {
             const int rp = (ho + g->pad_t) & 1, sp = (wo + g->pad_l) & 1;
-            if (rp >= g->R || sp >= g->S) need_zero = true;
+            if (rp >= g->R || sp >= g->S) empty |= 1u << (ho * 2 + wo);
         }
-    if (need_zero) SAE_CUDA_TRY(cudaMemsetAsync(dx, 0, (size_t)g->N * g->H * g->W * g->C * sizeof(float), st));
+    if (empty) {
+        const int64_t total = (int64_t)g->N * g->H * g->W * g->C;
+        if (!e.bias && !e.noise && !e.residual && !e.act_mask) {
+            SAE_CUDA_TRY(cudaMemsetAsync(dx, 0, (size_t)total * sizeof(float), st));
+        } else {
+            int64_t blocks = (total + 255) / 256;
+            if (blocks > (int64_t)sm_count() * 16) blocks = (int64_t)sm_count() * 16;
+            tc_dgrad_empty_kernel<<<(unsigned)blocks, 256, 0, st>>>(dx, e, total, g->H, g->W, g->C, empty);
+            int rc = check_launch("conv_wg(dgrad, empty parity classes)");
+            if (rc) return rc;
+        }
+    }
     TcProblem cls_pr[TC_MAX_BATCH];
     int ncls = 0;
     for (int ho = 0; ho < 2; ++ho)
