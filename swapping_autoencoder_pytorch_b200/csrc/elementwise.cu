@@ -497,7 +497,10 @@ extern "C" int sae_fused_bias_act(const float* x, const float* bias, const float
     if (!bias) { size_b = 1; step_b = 1; }
     cudaStream_t st = (cudaStream_t)stream;
     uintptr_t al = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(ref);
-    bool vec = (size_x % 4 == 0) && (al % 16 == 0) && (!noise || noise_div % 4 == 0);
+    // The float4 kernel wraps the channel cb + j (j < 4) with one subtraction when channels are innermost.  That is right for
+    // size_b >= 3 (cb + j <= size_b + 2 < 2 size_b) and for size_b == 2 (cb is even).  One channel would read b[1..3]: scalar.
+    const bool one_channel = bias && step_b == 1 && size_b == 1;
+    bool vec = (size_x % 4 == 0) && (al % 16 == 0) && (!noise || noise_div % 4 == 0) && !one_channel;
     const bool small = size_x < ((int64_t)1 << 31) && step_b < ((int64_t)1 << 31);      // 32-bit index arithmetic
     if (vec) {
         int64_t nv = size_x / 4;
