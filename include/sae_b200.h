@@ -31,7 +31,7 @@ extern "C" {
 #define SAE_E_UNSUPPORTED  -3   /* valid request this build has no kernel for                */
 
 /* ABI version of this header; bumped on any signature change. */
-#define SAE_ABI_VERSION 14
+#define SAE_ABI_VERSION 15
 int         sae_abi_version(void);
 const char* sae_last_error(void);
 /* number of kernels launched by this library in the calling process since load
@@ -347,6 +347,60 @@ int sae_torgb_forward(const float* x, const float* s, const float* w, const floa
 int sae_torgb_backward(const float* dy, const float* x, const float* s, const float* w, float* dx, float* gw,
                        int N, int H, int W, int C, float wscale,
                        int64_t ds_n, int64_t ds_c, int64_t ds_h, int64_t ds_w, int round_tf32, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Deterministic mode.  The entry points above that sum across CTAs (the conv weight gradients, plain and modulated, the
+ * split K of the generic kernel's deep linears, the bias / noise-weight / style / ToRGB gradients) do so with fp32 atomics,
+ * whose order changes from run to run.  Each has a _det twin that takes the same arguments followed by (workspace,
+ * workspace_bytes) and returns bitwise reproducible results: the CTAs store
+ * their partial sums with plain stores into a slot-major workspace ws[slot][target], and one reduction kernel adds the
+ * slots into the destination in slot order.  The partition is a pure function of the arguments (the planners assume a
+ * 132-SM H100 wherever the atomic twin reads the device's SM count), so results agree across runs, processes, CUDA-graph
+ * replay and H100 variants.  Outputs that the atomic twins accumulate into (dw, ds, grad_bias, grad_noise_weight, gw) are
+ * still accumulated into.  "The arguments" include the data pointers' 16-byte alignment, which selects the vectorised or
+ * the wgmma path where the atomic twin's choice depends on it: query with the pointers (or pointers of the same alignment)
+ * of the real call.
+ * Two-phase calls, as in CUB: with workspace == NULL the twin validates its arguments, stores the workspace size it needs in
+ * *workspace_bytes and returns SAE_OK without any CUDA call (the data pointers are not dereferenced).  Then call again with a
+ * device buffer of at least that many bytes (any size, even 0, wants a non-NULL pointer); a smaller *workspace_bytes
+ * returns SAE_E_INVALID.  The workspace may be reused once the stream has passed the call.  Results are deterministic for a
+ * fixed build, arguments and workspace-size query; they are not bitwise equal to the atomic twins'.
+ * ------------------------------------------------------------------------------------------ */
+int sae_conv2d_fprop_det(const float* x, const float* w, float* y, const sae_conv_geom* g, const sae_conv_epilogue* epi,
+                         int impl, void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_conv2d_dgrad_det(const float* dy, const float* wt, float* dx, const sae_conv_geom* g, const sae_conv_epilogue* epi,
+                         int impl, void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_conv2d_wgrad_det(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl,
+                         void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_conv2d_fprop_3xtf32_det(const float* x, const float* w_hi, const float* w_lo, float* y, const sae_conv_geom* g,
+                                const sae_conv_epilogue* epi, int impl, void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_conv2d_dgrad_3xtf32_det(const float* dy, const float* wt_hi, const float* wt_lo, float* dx, const sae_conv_geom* g,
+                                const sae_conv_epilogue* epi, int impl, void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_conv2d_wgrad_3xtf32_det(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl,
+                                void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_conv2d_wgrad_modulated_det(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
+                                   const sae_conv_geom* g, void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_conv2d_wgrad_modulated_3xtf32_det(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw,
+                                          float* ds, const sae_conv_geom* g, void* workspace, int64_t* workspace_bytes,
+                                          void* stream);
+/* The bandwidth-bound backward passes that reduce across CTAs (bias, noise-weight, style and ToRGB weight gradients), with
+ * the same protocol.  sae_fir_act_backward_det runs the FIR and then the activation backward as two passes (grad_in
+ * within one rounding of the fused kernel's); like its twin it returns SAE_E_UNSUPPORTED outside the fused configuration. */
+int sae_bias_act_backward_det(const float* grad_out, const float* out, float* grad_in, float* grad_bias,
+                              int64_t size_x, int size_b, float alpha, float scale,
+                              const float* noise, int64_t noise_div, float* grad_noise_weight,
+                              int round_tf32, const uint32_t* act_mask, void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_fir_act_backward_det(const float* grad, const float* taps_y, const float* taps_x, const float* act_out,
+                             float* grad_in, float* grad_bias, int64_t major, int in_h, int in_w, int minor,
+                             int kernel_h, int kernel_w, int pad_x0, int pad_x1, int pad_y0, int pad_y1,
+                             float alpha, float scale, int round_tf32, const uint32_t* act_mask,
+                             void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_modulate_backward_det(const float* dy, const float* x, const float* s, float* dx, float* ds,
+                              int n, int64_t hw, int c, int round_tf32, void* workspace, int64_t* workspace_bytes, void* stream);
+int sae_torgb_backward_det(const float* dy, const float* x, const float* s, const float* w, float* dx, float* gw,
+                           int N, int H, int W, int C, float wscale,
+                           int64_t ds_n, int64_t ds_c, int64_t ds_h, int64_t ds_w, int round_tf32,
+                           void* workspace, int64_t* workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsae_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
 
-SAE_ABI_VERSION = 14
+SAE_ABI_VERSION = 15
 
 c_float_p = ctypes.c_void_p   # raw device pointers travel as integers
 c_stream = ctypes.c_void_p
@@ -118,6 +118,15 @@ SIGNATURES = {
     "sae_torgb_backward": (ctypes.c_int, [c_float_p] * 6 + [ctypes.c_int] * 4 + [ctypes.c_float] + [ctypes.c_int64] * 4
                            + [ctypes.c_int, c_stream]),
 }
+
+# deterministic twins (header: "Deterministic mode"): the original arguments, then (workspace, int64_t* workspace_bytes)
+_WS = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]
+for _name in ("sae_conv2d_fprop", "sae_conv2d_dgrad", "sae_conv2d_wgrad", "sae_conv2d_fprop_3xtf32", "sae_conv2d_dgrad_3xtf32",
+              "sae_conv2d_wgrad_3xtf32", "sae_conv2d_wgrad_modulated", "sae_conv2d_wgrad_modulated_3xtf32",
+              "sae_bias_act_backward", "sae_fir_act_backward", "sae_modulate_backward", "sae_torgb_backward"):
+    _res, _args = SIGNATURES[_name]
+    SIGNATURES[_name + "_det"] = (_res, _args[:-1] + _WS + [c_stream])
+DET_ENTRY_POINTS = tuple(n for n in SIGNATURES if n.endswith("_det"))
 
 _lib = None
 _lock = threading.Lock()

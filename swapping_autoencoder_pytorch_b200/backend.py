@@ -40,6 +40,14 @@ def parse_precision(value):
     return v
 
 
+def parse_deterministic(value):
+    """``SAE_DETERMINISTIC`` value -> bool: unset, "" or "0" off, "1" on; anything else raises ValueError"""
+    v = "" if value is None else str(value).strip()
+    if v not in ("", "0", "1"):
+        raise ValueError("unknown SAE_DETERMINISTIC value %r: expected 0 or 1" % (value,))
+    return v == "1"
+
+
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
@@ -132,6 +140,11 @@ class CudaKernels:
         # fp32-accurate products at about a third of the TF32 tensor-core rate, and nothing is rounded to TF32 on storage
         # (every round_tf32 argument is 0).  The torch flags (cudnn.allow_tf32, matmul.allow_tf32) are not consulted.
         self.precision = os.environ.get("SAE_PRECISION")
+        # Deterministic mode: every gradient reduction runs through the _det twin of its entry point, which adds the CTAs'
+        # partial sums in a fixed order instead of with fp32 atomics, so training steps are bitwise reproducible (run to run,
+        # eager against CUDA-graph replay, on any H100).  torch.use_deterministic_algorithms(True) turns it on as well: see
+        # deterministic_mode().
+        self.deterministic = parse_deterministic(os.environ.get("SAE_DETERMINISTIC"))
 
     @property
     def precision(self):
@@ -140,6 +153,23 @@ class CudaKernels:
     @precision.setter
     def precision(self, value):
         self._precision = parse_precision(value)
+
+    def deterministic_mode(self):
+        """the effective mode: this object's flag or torch.use_deterministic_algorithms"""
+        return bool(self.deterministic) or torch.are_deterministic_algorithms_enabled()
+
+    def _call(self, name, *args):
+        """``name(*args, stream)``, or in deterministic mode its _det twin: a size query, then the call with a workspace from
+        the caching allocator (stream-ordered: the memory is reused only by work queued after this call)"""
+        if not self.deterministic_mode():
+            return getattr(self.lib, name)(*args, _stream())
+        fn = getattr(self.lib, name + "_det")
+        size = ctypes.c_int64(0)
+        rc = fn(*args, None, ctypes.byref(size), None)
+        if rc != 0:
+            return rc
+        ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=torch.device("cuda", torch.cuda.current_device()))
+        return fn(*args, _ptr(ws), ctypes.byref(size), _stream())
 
     def _round(self, flag=None):
         """the round_tf32 argument of a kernel call: the policy flag (or an explicit per-call value), always 0 in fp32 mode"""
@@ -203,9 +233,8 @@ class CudaKernels:
         gb = torch.zeros(c, device=out.device, dtype=out.dtype) if want_bias else None
         gnw = torch.zeros(1, device=out.device, dtype=out.dtype) if noise is not None else None
         with torch.cuda.device(out.device):
-            check(self.lib.sae_bias_act_backward(_ptr(grad_out), _ptr(out), _ptr(gi), _ptr(gb), out.numel(), c,
-                                                 alpha, scale, _ptr(noise), c, _ptr(gnw), self._round(), _ptr(mask), _stream()),
-                  "sae_bias_act_backward")
+            check(self._call("sae_bias_act_backward", _ptr(grad_out), _ptr(out), _ptr(gi), _ptr(gb), out.numel(), c,
+                             alpha, scale, _ptr(noise), c, _ptr(gnw), self._round(), _ptr(mask)), "sae_bias_act_backward")
         return gi, gb, gnw
 
     def fir_act_backward(self, grad, taps, act_out, pad, alpha, scale, want_bias=True, mask=None):
@@ -225,8 +254,8 @@ class CudaKernels:
         ty = (ctypes.c_float * kh)(*taps[0])
         tx = (ctypes.c_float * kw)(*taps[1])
         with torch.cuda.device(grad.device):
-            rc = self.lib.sae_fir_act_backward(_ptr(grad), ty, tx, _ptr(act_out), _ptr(gi), _ptr(gb), n, h, w, c, kh, kw,
-                                               px0, px1, py0, py1, alpha, scale, self._round(), _ptr(mask), _stream())
+            rc = self._call("sae_fir_act_backward", _ptr(grad), ty, tx, _ptr(act_out), _ptr(gi), _ptr(gb), n, h, w, c, kh, kw,
+                            px0, px1, py0, py1, alpha, scale, self._round(), _ptr(mask))
         if rc == -3:            # SAE_E_UNSUPPORTED: e.g. no TMA on this device
             return None
         check(rc, "sae_fir_act_backward")
@@ -273,8 +302,8 @@ class CudaKernels:
         dx = torch.empty_like(x)
         ds = torch.zeros_like(s)
         with torch.cuda.device(x.device):
-            check(self.lib.sae_modulate_backward(_ptr(dy), _ptr(x), _ptr(s), _ptr(dx), _ptr(ds), n, h * w, c,
-                                                 self._round(), _stream()), "sae_modulate_backward")
+            check(self._call("sae_modulate_backward", _ptr(dy), _ptr(x), _ptr(s), _ptr(dx), _ptr(ds), n, h * w, c,
+                             self._round()), "sae_modulate_backward")
         return dx, ds
 
     # ------------------------------------------------------- residual merge
@@ -408,10 +437,10 @@ class CudaKernels:
         with torch.cuda.device(x.device):
             if self._precision == "fp32":
                 hi, lo = self.split_tf32(w_krsc)
-                check(self.lib.sae_conv2d_fprop_3xtf32(_ptr(x), _ptr(hi), _ptr(lo), _ptr(y), ctypes.byref(g), ctypes.byref(e), impl,
-                                                       _stream()), "sae_conv2d_fprop_3xtf32")
+                check(self._call("sae_conv2d_fprop_3xtf32", _ptr(x), _ptr(hi), _ptr(lo), _ptr(y), ctypes.byref(g), ctypes.byref(e),
+                                 impl), "sae_conv2d_fprop_3xtf32")
             else:
-                check(self.lib.sae_conv2d_fprop(_ptr(x), _ptr(w_krsc), _ptr(y), ctypes.byref(g), ctypes.byref(e), impl, _stream()),
+                check(self._call("sae_conv2d_fprop", _ptr(x), _ptr(w_krsc), _ptr(y), ctypes.byref(g), ctypes.byref(e), impl),
                       "sae_conv2d_fprop")
         if mask is not None:
             y._sae_act_mask = mask
@@ -430,10 +459,10 @@ class CudaKernels:
         with torch.cuda.device(dy.device):
             if self._precision == "fp32":
                 hi, lo = self.split_tf32(wt)
-                check(self.lib.sae_conv2d_dgrad_3xtf32(_ptr(dy), _ptr(hi), _ptr(lo), _ptr(dx), ctypes.byref(g), ctypes.byref(e), impl,
-                                                       _stream()), "sae_conv2d_dgrad_3xtf32")
+                check(self._call("sae_conv2d_dgrad_3xtf32", _ptr(dy), _ptr(hi), _ptr(lo), _ptr(dx), ctypes.byref(g), ctypes.byref(e),
+                                 impl), "sae_conv2d_dgrad_3xtf32")
             else:
-                check(self.lib.sae_conv2d_dgrad(_ptr(dy), _ptr(wt), _ptr(dx), ctypes.byref(g), ctypes.byref(e), impl, _stream()),
+                check(self._call("sae_conv2d_dgrad", _ptr(dy), _ptr(wt), _ptr(dx), ctypes.byref(g), ctypes.byref(e), impl),
                       "sae_conv2d_dgrad")
         return dx
 
@@ -443,10 +472,9 @@ class CudaKernels:
         assert tuple(dy.shape) == (g.N, g.P, g.Q, g.K) and tuple(x.shape) == (g.N, g.H, g.W, g.C), \
             (tuple(dy.shape), tuple(x.shape), g.key())
         dw = torch.zeros((g.K, g.R, g.S, g.C), device=dy.device, dtype=dy.dtype)
-        fn, name = ((self.lib.sae_conv2d_wgrad_3xtf32, "sae_conv2d_wgrad_3xtf32") if self._precision == "fp32"
-                    else (self.lib.sae_conv2d_wgrad, "sae_conv2d_wgrad"))
+        name = "sae_conv2d_wgrad_3xtf32" if self._precision == "fp32" else "sae_conv2d_wgrad"
         with torch.cuda.device(dy.device):
-            check(fn(_ptr(dy), _ptr(x), _ptr(dw), ctypes.byref(g), self.conv_impl if impl is None else impl, _stream()), name)
+            check(self._call(name, _ptr(dy), _ptr(x), _ptr(dw), ctypes.byref(g), self.conv_impl if impl is None else impl), name)
         return dw
 
     # ------------------------------------------------ style-modulated conv, per-sample filters
@@ -504,10 +532,9 @@ class CudaKernels:
         _need_cuda(dy, x, s, w_krsc)
         dw = torch.zeros((g.K, g.R, g.S, g.C), device=dy.device, dtype=dy.dtype)
         ds = torch.zeros((g.N, g.C), device=dy.device, dtype=dy.dtype)
-        fn, name = ((self.lib.sae_conv2d_wgrad_modulated_3xtf32, "sae_conv2d_wgrad_modulated_3xtf32") if self._precision == "fp32"
-                    else (self.lib.sae_conv2d_wgrad_modulated, "sae_conv2d_wgrad_modulated"))
+        name = "sae_conv2d_wgrad_modulated_3xtf32" if self._precision == "fp32" else "sae_conv2d_wgrad_modulated"
         with torch.cuda.device(dy.device):
-            check(fn(_ptr(dy), _ptr(x), _ptr(s), _ptr(w_krsc), _ptr(dw), _ptr(ds), ctypes.byref(g), _stream()), name)
+            check(self._call(name, _ptr(dy), _ptr(x), _ptr(s), _ptr(w_krsc), _ptr(dw), _ptr(ds), ctypes.byref(g)), name)
         return dw, ds
 
     def conv_impl_for(self, g, direction):
@@ -562,9 +589,8 @@ class CudaKernels:
         dx = torch.empty_like(x) if want_dx else None
         gw = torch.zeros((n, 3, c), device=x.device, dtype=x.dtype) if want_gw else None
         with torch.cuda.device(x.device):
-            check(self.lib.sae_torgb_backward(_ptr(dy), _ptr(x), _ptr(s), _ptr(w), _ptr(dx), _ptr(gw), n, h, wd, c, wscale,
-                                              dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3), self._round(),
-                                              _stream()), "sae_torgb_backward")
+            check(self._call("sae_torgb_backward", _ptr(dy), _ptr(x), _ptr(s), _ptr(w), _ptr(dx), _ptr(gw), n, h, wd, c, wscale,
+                             dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3), self._round()), "sae_torgb_backward")
         return dx, gw
 
     # ----------------------------------------------------------------- crops

@@ -39,6 +39,40 @@ inline int check_launch(const char* what) {
 // process drives one GPU in this design).
 int sm_count();
 
+// ---- deterministic mode (the _det entry points) ---------------------------------------------------------------------------
+// Every cross-CTA sum is split into slots: each CTA stores its partial with plain stores into a slot-major workspace
+// ws[slot][target], and det_reduce adds the slots into the destination in slot order.  Partitions are planned with DET_SMS in
+// place of sm_count(), so the order of every addition is a function of the call's arguments alone.
+constexpr int DET_SMS = 132;
+
+// workspace regions start on 256-byte boundaries
+inline int64_t det_region(int64_t floats) { return (floats * 4 + 255) & ~(int64_t)255; }
+
+// The two-phase workspace protocol: workspace == NULL stores `need` in *workspace_bytes and sets *query; a workspace smaller
+// than `need` is refused.  No CUDA call is made either way.
+inline int det_workspace(const void* workspace, int64_t* workspace_bytes, int64_t need, const char* who, bool* query) {
+    *query = false;
+    if (!workspace_bytes) return fail(SAE_E_INVALID, "%s: null workspace_bytes", who);
+    if (!workspace) {
+        *workspace_bytes = need;
+        *query = true;
+        return SAE_OK;
+    }
+    if (*workspace_bytes < need)
+        return fail(SAE_E_INVALID, "%s: workspace of %lld bytes, %lld needed", who, (long long)*workspace_bytes, (long long)need);
+    return SAE_OK;
+}
+
+// dst[i] (+)= sum_{s < slots} ws[s * n + i], slots added in order; accumulate = 0 overwrites dst; round_tf32 rounds the result
+int det_reduce(float* dst, const float* ws, int64_t slots, int64_t n, bool accumulate, int round_tf32, cudaStream_t st);
+
+// a drain's contribution: an fp32 atomic into the destination, or (DET) a plain store into the CTA's workspace slot
+template <bool DET>
+__device__ __forceinline__ void drain_add(float* p, float v) {
+    if constexpr (DET) *p = v;
+    else atomicAdd(p, v);
+}
+
 __device__ __forceinline__ float rna_tf32(float v) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));

@@ -58,7 +58,29 @@ __device__ __forceinline__ void mma_tf32_3x(float (&acc)[4], const uint32_t (&ah
 }
 
 // ------------------------------------------------------------------------------------------------
-template <int BN, bool VEC, bool SPLIT>
+// ------------------------------------------------------------------------------------------------ deterministic slot reduction
+// dst[i] (+)= ws[0][i] + ws[1][i] + ... in slot order: the reduction behind every _det entry point
+__global__ void __launch_bounds__(256)
+det_reduce_kernel(float* __restrict__ dst, const float* __restrict__ ws, int64_t slots, int64_t n, int accumulate, int round_tf32) {
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        float v = ws[i];
+        for (int64_t s = 1; s < slots; ++s) v += ws[s * n + i];
+        if (accumulate) v = dst[i] + v;
+        dst[i] = round_tf32 ? rna_tf32(v) : v;
+    }
+}
+
+int det_reduce(float* dst, const float* ws, int64_t slots, int64_t n, bool accumulate, int round_tf32, cudaStream_t st) {
+    if (n == 0 || slots == 0) return SAE_OK;
+    int64_t blocks = (n + 255) / 256;
+    if (blocks > (int64_t)DET_SMS * 16) blocks = (int64_t)DET_SMS * 16;
+    det_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(dst, ws, slots, n, accumulate ? 1 : 0, round_tf32);
+    return check_launch("det_reduce");
+}
+
+// ------------------------------------------------------------------------------------------------
+// DET (split-K only): `out` is the workspace, one [M, Ncol] slab per K split (slot = blockIdx.z), written with plain stores
+template <int BN, bool VEC, bool SPLIT, bool DET>
 __global__ void __launch_bounds__(NTHREADS)
 conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat, float* __restrict__ out,
                    GatherParams p, EpiParams e, const float* __restrict__ wlo) {
@@ -255,6 +277,7 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
 
     // epilogue (split-K runs only with the plain epilogue; launch_gather applies round_tf32 to the summed output)
     if (split) {
+        float* const outz = DET ? out + (int64_t)blockIdx.z * p.M * p.Ncol : out;
 #pragma unroll
         for (int i = 0; i < MT; ++i)
 #pragma unroll
@@ -266,7 +289,7 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
 #pragma unroll
                     for (int u = 0; u < 2; ++u) {
                         int col = n0 + wn * 32 + j * 8 + 2 * t + u;
-                        if (col < p.Ncol) atomicAdd(out + m * p.Ncol + col, acc[i][j][h * 2 + u]);
+                        if (col < p.Ncol) drain_add<DET>(outz + m * p.Ncol + col, acc[i][j][h * 2 + u]);
                     }
             }
         return;
@@ -332,7 +355,9 @@ conv_gather_kernel(const float* __restrict__ src, const float* __restrict__ wmat
 // ------------------------------------------------------------------------------------------------
 constexpr int LDS_M = 128 + 8;
 
-template <bool VA, bool VB, bool SPLIT>
+// DET: dw is the workspace's dW region, one [Ko, Ncol] slab per pixel split (slot = blockIdx.z), and p.mod_ds its ds region
+// (N * C floats per slot, row group = one warp row of 64 output channels: see wgrad_ds_slot)
+template <bool VA, bool VB, bool SPLIT, bool DET>
 __global__ void __launch_bounds__(NTHREADS)
 conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, float* __restrict__ dw, WgradParams p) {
     extern __shared__ __align__(16) float smem[];
@@ -500,6 +525,7 @@ conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, flo
     }
     cp_async_wait<0>();
 
+    float* const dwz = DET ? dw + (int64_t)blockIdx.z * p.Ko * p.Ncol : dw;
     if (p.img_pix > 0) {
         const int img = (int)(pix0 / p.img_pix);
 #pragma unroll
@@ -519,13 +545,20 @@ conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, flo
                         if (o >= p.Ko || !nok) continue;
                         const float v = acc[i][j][h * 2 + u];
                         dsum += v * __ldg(p.mod_w + (int64_t)o * p.Ncol + n);
-                        atomicAdd(dw + (int64_t)o * p.Ncol + n, v * sc);
+                        drain_add<DET>(dwz + (int64_t)o * p.Ncol + n, v * sc);
                     }
                 // the 8 lanes of a column (g = 0..7) share n: reduce before the atomic
                 dsum += __shfl_xor_sync(0xffffffffu, dsum, 4);
                 dsum += __shfl_xor_sync(0xffffffffu, dsum, 8);
                 dsum += __shfl_xor_sync(0xffffffffu, dsum, 16);
-                if (g == 0 && nok) atomicAdd(p.mod_ds + (int64_t)img * p.C + c, dsum);
+                if constexpr (DET) {
+                    const int64_t spi = p.img_pix / p.chunk;
+                    if (g == 0 && nok)
+                        p.mod_ds[wgrad_ds_slot(2 * blockIdx.x + wm, blockIdx.z - img * spi, spi, n / p.C, p.Ncol / p.C) *
+                                     ((int64_t)p.N * p.C) + (int64_t)img * p.C + c] = dsum;
+                } else {
+                    if (g == 0 && nok) atomicAdd(p.mod_ds + (int64_t)img * p.C + c, dsum);
+                }
             }
         return;
     }
@@ -540,50 +573,60 @@ conv_wgrad_kernel(const float* __restrict__ dy, const float* __restrict__ x, flo
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
                     int n = n0 + wn * 32 + j * 8 + 2 * t + u;
-                    if (n < p.Ncol) atomicAdd(dw + (int64_t)o * p.Ncol + n, acc[i][j][h * 2 + u]);
+                    if (n < p.Ncol) drain_add<DET>(dwz + (int64_t)o * p.Ncol + n, acc[i][j][h * 2 + u]);
                 }
         }
 }
 
 // ------------------------------------------------------------------------------------------------
-template <int BN, bool VEC, bool SPLIT>
+// K splits of the gather GEMM: small-M, deep-K problems (linears) split K so more than a handful of SMs work on them
+static unsigned gather_ksplits(const GatherParams& p, const EpiParams& e, int BN) {
+    const int64_t tiles = ((p.M + BM - 1) / BM) * ((p.Ncol + BN - 1) / BN);
+    const int kblocks = (p.K + BK - 1) / BK;
+    const bool plain = !e.bias && !e.noise && !e.residual && e.act == 1 && e.gain == 1.f;
+    if (!(plain && tiles <= 16 && kblocks >= 16)) return 1;
+    unsigned z = (unsigned)(kblocks / 4);
+    if (z > 32) z = 32;
+    return z > 1 ? z : 1;
+}
+
+// det_ws non-null (the deterministic twin): the split-K partials go to det_ws and det_reduce sums them in split order,
+// rounding to TF32 on the way when the epilogue asks for it (no memset, no atomics, no separate rounding pass)
+template <int BN, bool VEC, bool SPLIT, bool DET = false>
 static int launch_gather(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
-                         cudaStream_t st, const float* wlo) {
+                         cudaStream_t st, const float* wlo, float* det_ws = nullptr) {
     size_t smem = (size_t)STAGES * (BM + (SPLIT ? 2 : 1) * BN) * LDS_K * sizeof(float);
     static bool attr_done = false;   // benign race: idempotent
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_gather_kernel<BN, VEC, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_gather_kernel<BN, VEC, SPLIT, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done = true;
     }
     dim3 grid((unsigned)((p.M + BM - 1) / BM), (unsigned)((p.Ncol + BN - 1) / BN));
-    // small-M, deep-K problems (linears): split K so more than a handful of SMs work on them
-    const int kblocks = (p.K + BK - 1) / BK;
-    const bool plain = !e.bias && !e.noise && !e.residual && e.act == 1 && e.gain == 1.f;
-    if (plain && grid.x * grid.y <= 16 && kblocks >= 16) {
-        unsigned z = (unsigned)(kblocks / 4);
-        if (z > 32) z = 32;
-        if (z > 1) {
-            grid.z = z;
-            SAE_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)p.M * p.Ncol * sizeof(float), st));
-        }
+    grid.z = gather_ksplits(p, e, BN);
+    if constexpr (DET) {
+        conv_gather_kernel<BN, VEC, SPLIT, true><<<grid, NTHREADS, smem, st>>>(src, wmat, grid.z > 1 ? det_ws : out, p, e, wlo);
+        int rc = check_launch("conv_gather_det");
+        if (rc == SAE_OK && grid.z > 1) rc = det_reduce(out, det_ws, grid.z, p.M * p.Ncol, false, e.round_tf32, st);
+        return rc;
     }
-    conv_gather_kernel<BN, VEC, SPLIT><<<grid, NTHREADS, smem, st>>>(src, wmat, out, p, e, wlo);
+    if (grid.z > 1) SAE_CUDA_TRY(cudaMemsetAsync(out, 0, (size_t)p.M * p.Ncol * sizeof(float), st));
+    conv_gather_kernel<BN, VEC, SPLIT, false><<<grid, NTHREADS, smem, st>>>(src, wmat, out, p, e, wlo);
     int rc = check_launch("conv_gather");
     // the split-K CTAs add raw partial sums into out: round the finished sums once they are all in
     if (rc == SAE_OK && grid.z > 1 && e.round_tf32) rc = sae_round_tf32(out, out, p.M * p.Ncol, st);
     return rc;
 }
 
-template <bool SPLIT>
+template <bool SPLIT, bool DET = false>
 static int gather_dispatch_t(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
-                             cudaStream_t st, const float* wlo) {
+                             cudaStream_t st, const float* wlo, float* det_ws = nullptr) {
     const bool aligned = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(wmat) | reinterpret_cast<uintptr_t>(wlo)) & 15) == 0;
     const bool vec = (p.Cs % 4 == 0) && aligned;
     if (p.Ncol > 64)
-        return vec ? launch_gather<128, true, SPLIT>(src, wmat, out, p, e, st, wlo) : launch_gather<128, false, SPLIT>(src, wmat, out, p, e, st, wlo);
+        return vec ? launch_gather<128, true, SPLIT, DET>(src, wmat, out, p, e, st, wlo, det_ws) : launch_gather<128, false, SPLIT, DET>(src, wmat, out, p, e, st, wlo, det_ws);
     if (p.Ncol > 32)
-        return vec ? launch_gather<64, true, SPLIT>(src, wmat, out, p, e, st, wlo) : launch_gather<64, false, SPLIT>(src, wmat, out, p, e, st, wlo);
-    return vec ? launch_gather<32, true, SPLIT>(src, wmat, out, p, e, st, wlo) : launch_gather<32, false, SPLIT>(src, wmat, out, p, e, st, wlo);
+        return vec ? launch_gather<64, true, SPLIT, DET>(src, wmat, out, p, e, st, wlo, det_ws) : launch_gather<64, false, SPLIT, DET>(src, wmat, out, p, e, st, wlo, det_ws);
+    return vec ? launch_gather<32, true, SPLIT, DET>(src, wmat, out, p, e, st, wlo, det_ws) : launch_gather<32, false, SPLIT, DET>(src, wmat, out, p, e, st, wlo, det_ws);
 }
 
 int conv_gather_dispatch(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
@@ -592,30 +635,43 @@ int conv_gather_dispatch(const float* src, const float* wmat, float* out, const 
     return wlo ? gather_dispatch_t<true>(src, wmat, out, p, e, st, wlo) : gather_dispatch_t<false>(src, wmat, out, p, e, st, nullptr);
 }
 
-template <bool VA, bool VB, bool SPLIT>
+int conv_gather_dispatch_det(const float* src, const float* wmat, float* out, const GatherParams& p, const EpiParams& e,
+                             cudaStream_t st, const float* wlo, void* ws, int64_t* ws_bytes, const char* who) {
+    const int BN = p.Ncol > 64 ? 128 : p.Ncol > 32 ? 64 : 32;
+    const unsigned z = (p.M == 0 || p.Ncol == 0) ? 1 : gather_ksplits(p, e, BN);
+    bool query;
+    int rc = det_workspace(ws, ws_bytes, z > 1 ? det_region((int64_t)z * p.M * p.Ncol) : 0, who, &query);
+    if (rc || query || p.M == 0 || p.Ncol == 0) return rc;
+    float* w = static_cast<float*>(ws);
+    return wlo ? gather_dispatch_t<true, true>(src, wmat, out, p, e, st, wlo, w) : gather_dispatch_t<false, true>(src, wmat, out, p, e, st, nullptr, w);
+}
+
+template <bool VA, bool VB, bool SPLIT, bool DET>
 static int launch_wgrad(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st) {
     size_t smem = (size_t)STAGES * 2 * BK * LDS_M * sizeof(float);
     static bool attr_done = false;
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_wgrad_kernel<VA, VB, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(conv_wgrad_kernel<VA, VB, SPLIT, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_done = true;
     }
     dim3 grid((unsigned)((p.Ko + 127) / 128), (unsigned)((p.Ncol + 127) / 128), splits);
-    conv_wgrad_kernel<VA, VB, SPLIT><<<grid, NTHREADS, smem, st>>>(dy, x, dw, p);
-    return check_launch("conv_wgrad");
+    conv_wgrad_kernel<VA, VB, SPLIT, DET><<<grid, NTHREADS, smem, st>>>(dy, x, dw, p);
+    return check_launch(DET ? "conv_wgrad_det" : "conv_wgrad");
 }
 
-template <bool SPLIT>
+template <bool SPLIT, bool DET>
 static int launch_wgrad_any(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st,
                             bool va, bool vb) {
-    if (va && vb) return launch_wgrad<true, true, SPLIT>(dy, x, dw, p, splits, st);
-    if (va) return launch_wgrad<true, false, SPLIT>(dy, x, dw, p, splits, st);
-    if (vb) return launch_wgrad<false, true, SPLIT>(dy, x, dw, p, splits, st);
-    return launch_wgrad<false, false, SPLIT>(dy, x, dw, p, splits, st);
+    if (va && vb) return launch_wgrad<true, true, SPLIT, DET>(dy, x, dw, p, splits, st);
+    if (va) return launch_wgrad<true, false, SPLIT, DET>(dy, x, dw, p, splits, st);
+    if (vb) return launch_wgrad<false, true, SPLIT, DET>(dy, x, dw, p, splits, st);
+    return launch_wgrad<false, false, SPLIT, DET>(dy, x, dw, p, splits, st);
 }
 
+// det non-null: the deterministic twin.  Its splits are planned for DET_SMS SMs, the wgmma kernels are taken as available
+// (the library runs on sm_90a only; a device without TMA makes the launch fail), and det->ws == nullptr only plans.
 static int wgrad_impl(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st,
-                      const float* mod_s, const float* mod_w, float* mod_ds, bool split) {
+                      const float* mod_s, const float* mod_w, float* mod_ds, bool split, DetWs* det = nullptr) {
     WgradParams p;
     p.mod_s = mod_s; p.mod_w = mod_w; p.mod_ds = mod_ds;
     p.img_pix = mod_s ? (int64_t)g->P * g->Q : 0;
@@ -625,10 +681,11 @@ static int wgrad_impl(const float* dy, const float* x, float* dw, const sae_conv
     p.Mpix = (int64_t)g->N * g->P * g->Q;
     if (p.Mpix == 0 || p.Ko == 0 || p.Ncol == 0) return SAE_OK;
     const bool al = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) == 0;
-    const bool wg_ok = impl != 1 && al && wgrad_wg_eligible(g) && tc_available();
-    if (wg_ok && !split) return wgrad_wg_launch(dy, x, dw, p, st);
+    const bool wg_ok = impl != 1 && al && wgrad_wg_eligible(g) && (det || tc_available());
+    if (wg_ok && !split) return wgrad_wg_launch(dy, x, dw, p, st, det);
     int64_t tiles = (int64_t)((p.Ko + 127) / 128) * ((p.Ncol + 127) / 128);
-    int64_t want = ((int64_t)sm_count() * 2 + tiles - 1) / tiles;      // ~2 CTAs per SM
+    const int64_t sms = det ? DET_SMS : sm_count();
+    int64_t want = (sms * 2 + tiles - 1) / tiles;      // ~2 CTAs per SM
     int64_t kblocks = (p.Mpix + BK - 1) / BK;
     if (want > kblocks) want = kblocks;
     if (want < 1) want = 1;
@@ -639,12 +696,46 @@ static int wgrad_impl(const float* dy, const float* x, float* dw, const sae_conv
     p.chunk = kb_per * BK;
     unsigned splits = (unsigned)((p.Mpix + p.chunk - 1) / p.chunk);
     const bool va = (p.Ko % 4 == 0) && al, vb = (p.C % 4 == 0) && al;
+    if (det) {
+        det->dw_slots = splits;
+        det->ds_slots = p.img_pix > 0 ? wgrad_ds_slots((p.Ko + 127) / 128, wg_ok ? 1 : 2, p.img_pix / p.chunk, p.R * p.S) : 0;
+        if (!det->ws) return SAE_OK;
+        if (wg_ok) return wgrad_split_launch(dy, x, dw, p, splits, st, det);
+        p.mod_ds = det->ws_ds;
+        return split ? launch_wgrad_any<true, true>(dy, x, det->ws, p, splits, st, va, vb)
+                     : launch_wgrad_any<false, true>(dy, x, det->ws, p, splits, st, va, vb);
+    }
     if (wg_ok) return wgrad_split_launch(dy, x, dw, p, splits, st);
-    return split ? launch_wgrad_any<true>(dy, x, dw, p, splits, st, va, vb) : launch_wgrad_any<false>(dy, x, dw, p, splits, st, va, vb);
+    return split ? launch_wgrad_any<true, false>(dy, x, dw, p, splits, st, va, vb) : launch_wgrad_any<false, false>(dy, x, dw, p, splits, st, va, vb);
 }
 
 int conv_wgrad(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st, bool split) {
     return wgrad_impl(dy, x, dw, g, impl, st, nullptr, nullptr, nullptr, split);
+}
+
+// plan (DetWs slot counts -> workspace size), check the workspace, run the deterministic drains, then add the slots into dW
+// (and ds) in slot order
+static int wgrad_det(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
+                     const sae_conv_geom* g, int impl, cudaStream_t st, bool split, void* ws, int64_t* ws_bytes, const char* who) {
+    DetWs det;
+    int rc = wgrad_impl(dy, x, dw, g, impl, st, s, w_krsc, ds, split, &det);
+    if (rc) return rc;
+    const int64_t dw_n = (int64_t)g->K * g->R * g->S * g->C, ds_n = (int64_t)g->N * g->C;
+    const int64_t dw_bytes = det.dw_slots > 0 ? det_region(det.dw_slots * dw_n) : 0;
+    bool query;
+    rc = det_workspace(ws, ws_bytes, dw_bytes + (det.ds_slots > 0 ? det_region(det.ds_slots * ds_n) : 0), who, &query);
+    if (rc || query || det.dw_slots == 0) return rc;
+    det.ws = static_cast<float*>(ws);
+    det.ws_ds = reinterpret_cast<float*>(static_cast<char*>(ws) + dw_bytes);
+    rc = wgrad_impl(dy, x, dw, g, impl, st, s, w_krsc, ds, split, &det);
+    if (rc == SAE_OK) rc = det_reduce(dw, det.ws, det.dw_slots, dw_n, true, 0, st);
+    if (rc == SAE_OK && det.ds_slots > 0) rc = det_reduce(ds, det.ws_ds, det.ds_slots, ds_n, true, 0, st);
+    return rc;
+}
+
+int conv_wgrad_det(const float* dy, const float* x, float* dw, const sae_conv_geom* g, int impl, cudaStream_t st, bool split,
+                   void* ws, int64_t* ws_bytes, const char* who) {
+    return wgrad_det(dy, x, nullptr, nullptr, dw, nullptr, g, impl, st, split, ws, ws_bytes, who);
 }
 
 bool wgrad_modulated_eligible(const sae_conv_geom* g) {
@@ -659,6 +750,14 @@ int conv_wgrad_modulated(const float* dy, const float* x, const float* s, const 
     if (((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) != 0)
         return fail(SAE_E_INVALID, "modulated wgrad: pointers must be 16-byte aligned");
     return wgrad_impl(dy, x, dw, g, 0, st, s, w_krsc, ds, split);
+}
+
+int conv_wgrad_modulated_det(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
+                             const sae_conv_geom* g, cudaStream_t st, bool split, void* ws, int64_t* ws_bytes, const char* who) {
+    if (!wgrad_modulated_eligible(g)) return fail(SAE_E_UNSUPPORTED, "modulated wgrad: needs stride 1, Q %% 32 == 0, C and K %% 32 == 0");
+    if (((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x)) & 15) != 0)
+        return fail(SAE_E_INVALID, "modulated wgrad: pointers must be 16-byte aligned");
+    return wgrad_det(dy, x, s, w_krsc, dw, ds, g, 0, st, split, ws, ws_bytes, who);
 }
 
 }  // namespace sae

@@ -57,7 +57,11 @@ struct WgpArgs {
     CUtensorMap dy, x;
 };
 
-__global__ void __launch_bounds__(WGP_THREADS, 1) wgrad_wg_kernel(float* __restrict__ dw, const __grid_constant__ WgpArgs args) {
+// DET: dw is the workspace of the deterministic mode, one [Ko, Ncol] slab per pixel split (slot = blockIdx.z), and p.mod_ds
+// its ds region, ds_slab = N * C floats per slot (the slot map of wgrad_ds_slot); every element of a slot is stored exactly once
+template <bool DET>
+__global__ void __launch_bounds__(WGP_THREADS, 1)
+wgrad_wg_kernel(float* __restrict__ dw, const __grid_constant__ WgpArgs args, const int64_t ds_slab) {
     const WgpParams& p = args.p;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-byte alignment
@@ -208,6 +212,7 @@ __global__ void __launch_bounds__(WGP_THREADS, 1) wgrad_wg_kernel(float* __restr
 
     // accumulator fragment: rows g (+ 8) of warp w -> channels o0 + 32 (w / 2) + 4 c4a (c4b) + g % 4, columns n0 + 8 j + 2 t + {0, 1}
     const int oa = o0 + 32 * (warp >> 1) + 4 * c4a + (g & 3), ob = oa + 4;
+    float* const dwz = DET ? dw + (int64_t)blockIdx.z * p.Ko * p.Ncol : dw;
     if (p.img_boxes > 0) {
         const int img = (int)(b0 / p.img_boxes);
         // ds: each warp's column sums over its 16 rows (shuffles) land in dsp[warp][column]; then one thread per column adds the
@@ -229,7 +234,7 @@ __global__ void __launch_bounds__(WGP_THREADS, 1) wgrad_wg_kernel(float* __restr
                     if (o >= p.Ko || !nok) continue;
                     const float v = acc[4 * j + 2 * h + u];
                     dsum += v * __ldg(p.mod_w + (int64_t)o * p.Ncol + n);
-                    atomicAdd(dw + (int64_t)o * p.Ncol + n, v * sc);
+                    drain_add<DET>(dwz + (int64_t)o * p.Ncol + n, v * sc);
                 }
                 // the 8 lanes of a column (g = 0..7) share n
                 dsum += __shfl_xor_sync(0xffffffffu, dsum, 4);
@@ -243,7 +248,13 @@ __global__ void __launch_bounds__(WGP_THREADS, 1) wgrad_wg_kernel(float* __restr
             float v = 0.f;
 #pragma unroll
             for (int w = 0; w < 8; ++w) v += dsp[w * 128 + tid];
-            atomicAdd(p.mod_ds + (int64_t)img * p.C + (n0 + tid) % p.C, v);
+            const int n = n0 + tid;
+            if constexpr (DET) {
+                const int64_t spi = p.img_boxes / p.chunk;
+                p.mod_ds[wgrad_ds_slot(blockIdx.x, blockIdx.z - img * spi, spi, n / p.C, p.Ncol / p.C) * ds_slab + (int64_t)img * p.C + n % p.C] = v;
+            } else {
+                atomicAdd(p.mod_ds + (int64_t)img * p.C + n % p.C, v);
+            }
         }
         return;
     }
@@ -256,8 +267,8 @@ __global__ void __launch_bounds__(WGP_THREADS, 1) wgrad_wg_kernel(float* __restr
         for (int h = 0; h < 2; ++h) {
             const int o = h ? ob : oa;
             if (o >= p.Ko) continue;
-            atomicAdd(dw + (int64_t)o * p.Ncol + n, acc[4 * j + 2 * h]);
-            atomicAdd(dw + (int64_t)o * p.Ncol + n + 1, acc[4 * j + 2 * h + 1]);
+            drain_add<DET>(dwz + (int64_t)o * p.Ncol + n, acc[4 * j + 2 * h]);
+            drain_add<DET>(dwz + (int64_t)o * p.Ncol + n + 1, acc[4 * j + 2 * h + 1]);
         }
     }
 }
@@ -266,7 +277,7 @@ bool wgrad_wg_eligible(const sae_conv_geom* g) {
     return g->K % 32 == 0 && g->C % 32 == 0 && (g->stride == 1 || g->stride == 2) && g->pad_t <= 100 && g->pad_l <= 100;
 }
 
-int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& wp, cudaStream_t st) {
+int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParams& wp, cudaStream_t st, DetWs* det) {
     WgpArgs a;
     WgpParams& p = a.p;
     p.Ko = wp.Ko; p.C = wp.C; p.Ncol = wp.Ncol; p.S = wp.S;
@@ -287,7 +298,7 @@ int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParam
     // the fewest splits that fill >= 90 % of the last wave; at least 8 boxes (256 pixels) per CTA keep the 16K atomics of
     // a CTA's drain small against its MMA work
     const int64_t tiles = (int64_t)((p.Ko + 127) / 128) * ((p.Ncol + 127) / 128);
-    const int64_t sms = sm_count();
+    const int64_t sms = det ? DET_SMS : sm_count();
     const int64_t s_max = p.boxes / 8 > 1 ? p.boxes / 8 : 1;
     const int64_t s_min = (2 * sms + tiles - 1) / tiles;
     int64_t splits = s_max;
@@ -302,17 +313,33 @@ int wgrad_wg_launch(const float* dy, const float* x, float* dw, const WgradParam
     }
     splits = (p.boxes + p.chunk - 1) / p.chunk;
     if (splits > 65535) return fail(SAE_E_UNSUPPORTED, "wgrad: %lld pixel splits", (long long)splits);
+    if (det) {
+        det->dw_slots = splits;
+        det->ds_slots = p.img_boxes > 0 ? wgrad_ds_slots((p.Ko + 127) / 128, 1, p.img_boxes / p.chunk, wp.R * wp.S) : 0;
+        if (!det->ws) return SAE_OK;
+        dw = det->ws;
+        p.mod_ds = det->ws_ds;
+    }
     int rc = encode_act_map(&a.dy, dy, wp.N, wp.P, wp.Q, wp.Ko, p.tw, p.th, p.tn, 1);
     if (rc) return rc;
     rc = encode_act_map(&a.x, x, wp.N, wp.H, wp.W, wp.C, p.tw, p.th, p.tn, wp.stride);
     if (rc) return rc;
+    dim3 grid((unsigned)((p.Ko + 127) / 128), (unsigned)((p.Ncol + 127) / 128), (unsigned)splits);
+    if (det) {
+        static bool attr_det = false;
+        if (!attr_det) {
+            SAE_CUDA_TRY(cudaFuncSetAttribute(wgrad_wg_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WGP_SMEM));
+            attr_det = true;
+        }
+        wgrad_wg_kernel<true><<<grid, WGP_THREADS, WGP_SMEM, st>>>(dw, a, (int64_t)wp.N * wp.C);
+        return check_launch("wgrad_wg_det");
+    }
     static bool attr_done = false;
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(wgrad_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WGP_SMEM));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(wgrad_wg_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WGP_SMEM));
         attr_done = true;
     }
-    dim3 grid((unsigned)((p.Ko + 127) / 128), (unsigned)((p.Ncol + 127) / 128), (unsigned)splits);
-    wgrad_wg_kernel<<<grid, WGP_THREADS, WGP_SMEM, st>>>(dw, a);
+    wgrad_wg_kernel<false><<<grid, WGP_THREADS, WGP_SMEM, st>>>(dw, a, 0);
     return check_launch("wgrad_wg");
 }
 
@@ -328,6 +355,8 @@ __device__ __forceinline__ void cp_async16_wg(uint32_t s, const void* gmem, bool
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(pred ? 16 : 0));
 }
 
+// DET: as wgrad_wg_kernel (dw = the workspace's dW slabs, p.mod_ds its ds region with N * C floats per slot)
+template <bool DET>
 __global__ void __launch_bounds__(WGR_THREADS, 1)
 wgrad_split_kernel(const float* __restrict__ dy, const float* __restrict__ x, float* __restrict__ dw, const WgradParams p) {
     extern __shared__ uint8_t smem_raw[];
@@ -436,6 +465,7 @@ wgrad_split_kernel(const float* __restrict__ dy, const float* __restrict__ x, fl
 
     // accumulator fragment: rows o0 + r0 (+ 8), columns n0 + 8 j + 2 t + {0, 1}
     const int orow = o0 + r0;
+    float* const dwz = DET ? dw + (int64_t)blockIdx.z * p.Ko * p.Ncol : dw;
     if (p.img_pix > 0) {
         const int img = (int)(pix0 / p.img_pix);
         // ds: as in the TF32 kernel, one atomic per column and CTA
@@ -455,7 +485,7 @@ wgrad_split_kernel(const float* __restrict__ dy, const float* __restrict__ x, fl
                     if (o >= p.Ko || !nok) continue;
                     const float v = acc[4 * j + 2 * h + u];
                     dsum += v * __ldg(p.mod_w + (int64_t)o * p.Ncol + n);
-                    atomicAdd(dw + (int64_t)o * p.Ncol + n, v * sc);
+                    drain_add<DET>(dwz + (int64_t)o * p.Ncol + n, v * sc);
                 }
                 dsum += __shfl_xor_sync(0xffffffffu, dsum, 4);
                 dsum += __shfl_xor_sync(0xffffffffu, dsum, 8);
@@ -467,7 +497,14 @@ wgrad_split_kernel(const float* __restrict__ dy, const float* __restrict__ x, fl
             float v = 0.f;
 #pragma unroll
             for (int w = 0; w < 8; ++w) v += dsp[w * 128 + tid];
-            atomicAdd(p.mod_ds + (int64_t)img * p.C + (n0 + tid) % p.C, v);
+            const int n = n0 + tid;
+            if constexpr (DET) {
+                const int64_t spi = p.img_pix / p.chunk;
+                p.mod_ds[wgrad_ds_slot(blockIdx.x, blockIdx.z - img * spi, spi, n / p.C, p.Ncol / p.C) * ((int64_t)p.N * p.C) +
+                         (int64_t)img * p.C + n % p.C] = v;
+            } else {
+                atomicAdd(p.mod_ds + (int64_t)img * p.C + n % p.C, v);
+            }
         }
         return;
     }
@@ -478,21 +515,30 @@ wgrad_split_kernel(const float* __restrict__ dy, const float* __restrict__ x, fl
         for (int h = 0; h < 2; ++h) {
             const int o = orow + 8 * h;
             if (o >= p.Ko) continue;
-            if (n < p.Ncol) atomicAdd(dw + (int64_t)o * p.Ncol + n, acc[4 * j + 2 * h]);
-            if (n + 1 < p.Ncol) atomicAdd(dw + (int64_t)o * p.Ncol + n + 1, acc[4 * j + 2 * h + 1]);
+            if (n < p.Ncol) drain_add<DET>(dwz + (int64_t)o * p.Ncol + n, acc[4 * j + 2 * h]);
+            if (n + 1 < p.Ncol) drain_add<DET>(dwz + (int64_t)o * p.Ncol + n + 1, acc[4 * j + 2 * h + 1]);
         }
     }
 }
 
-int wgrad_split_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st) {
+template <bool DET>
+static int wgrad_split_launch_t(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st) {
     static bool attr_done = false;
     if (!attr_done) {
-        SAE_CUDA_TRY(cudaFuncSetAttribute(wgrad_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WGR_SMEM));
+        SAE_CUDA_TRY(cudaFuncSetAttribute(wgrad_split_kernel<DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WGR_SMEM));
         attr_done = true;
     }
     dim3 grid((unsigned)((p.Ko + 127) / 128), (unsigned)((p.Ncol + 127) / 128), splits);
-    wgrad_split_kernel<<<grid, WGR_THREADS, WGR_SMEM, st>>>(dy, x, dw, p);
-    return check_launch("wgrad_split");
+    wgrad_split_kernel<DET><<<grid, WGR_THREADS, WGR_SMEM, st>>>(dy, x, dw, p);
+    return check_launch(DET ? "wgrad_split_det" : "wgrad_split");
+}
+
+int wgrad_split_launch(const float* dy, const float* x, float* dw, const WgradParams& p, unsigned splits, cudaStream_t st,
+                       const DetWs* det) {
+    if (!det) return wgrad_split_launch_t<false>(dy, x, dw, p, splits, st);
+    WgradParams q = p;
+    q.mod_ds = det->ws_ds;
+    return wgrad_split_launch_t<true>(dy, x, det->ws, q, splits, st);
 }
 
 }  // namespace sae

@@ -30,7 +30,7 @@ class HalfStepGraphs:
         self.trainer = trainer
         self.warmup = warmup
         self.calls = {}
-        self.captured = {}        # (kind, input shape, kernel precision) -> (graph, static_input, static_outputs, launches)
+        self.captured = {}        # (kind, input shape, kernel precision, deterministic) -> (graph, static_input, static_outputs, launches)
         self.pool = None
         self.stream = None             # side stream shared by the eager warm-up calls and every capture (see _side)
         self.disabled = None
@@ -97,11 +97,14 @@ class HalfStepGraphs:
         if self.disabled is not None or not self.enabled:
             return body(images)
         # a graph records the kernels of one precision mode (backend.CudaKernels.precision): switching the mode captures new
-        # graphs, after warm-up calls of their own (the other mode's kernels initialise lazily, outside any capture)
-        precision = getattr(backend.kernels(), "precision", "tf32")
-        n = self.calls.get((kind, precision), 0)
-        self.calls[(kind, precision)] = n + 1
-        key = (kind, tuple(images.shape), precision)
+        # graphs, after warm-up calls of their own (the other mode's kernels initialise lazily, outside any capture).  The same
+        # holds for the deterministic mode (backend.CudaKernels.deterministic_mode()), which records other kernels.
+        k = backend.kernels()
+        precision = getattr(k, "precision", "tf32")
+        det = bool(getattr(k, "deterministic_mode", lambda: False)())
+        n = self.calls.get((kind, precision, det), 0)
+        self.calls[(kind, precision, det)] = n + 1
+        key = (kind, tuple(images.shape), precision, det)
         hit = self.captured.get(key)
         if hit is None:
             if n < self.warmup:
