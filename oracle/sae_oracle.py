@@ -355,13 +355,14 @@ class OracleModel:
         sp, gl = encoder_forward(self.E, self.opt, real)
         return generator_forward(self.G, self.opt, sp, gl)
 
-    def discriminator_losses(self, real):
-        """reference swapping_autoencoder_model.py:62-136"""
+    def discriminator_losses(self, real, noises=(None, None)):
+        """reference swapping_autoencoder_model.py:62-136.  ``noises``: the ``generator_forward`` noise dicts of the two G
+        calls (rec, mix); None draws fresh noise."""
         opt = self.opt
         b = real.size(0)
         sp, gl = encoder_forward(self.E, opt, real)
-        rec = generator_forward(self.G, opt, sp[:b // 2], gl[:b // 2])
-        mix = generator_forward(self.G, opt, swap(sp), gl)
+        rec = generator_forward(self.G, opt, sp[:b // 2], gl[:b // 2], noises[0])
+        mix = generator_forward(self.G, opt, swap(sp), gl, noises[1])
         L = {}
         if opt.lambda_GAN > 0:
             L["D_real"] = gan_loss(discriminator_forward(self.D, opt, real), True) * opt.lambda_GAN
@@ -396,12 +397,12 @@ class OracleModel:
             cpen = (g1.pow(2).sum(dims) + g2.pow(2).sum(dims)) * (0.5 * opt.lambda_patch_R1 * 0.5)
         return {"D_R1": pen + cpen}
 
-    def generator_losses(self, real):
-        """reference swapping_autoencoder_model.py:187-231"""
+    def generator_losses(self, real, noises=(None, None)):
+        """reference swapping_autoencoder_model.py:187-231.  ``noises`` as in ``discriminator_losses``."""
         opt = self.opt
         b = real.size(0)
         sp, gl = encoder_forward(self.E, opt, real)
-        rec = generator_forward(self.G, opt, sp[:b // 2], gl[:b // 2])
+        rec = generator_forward(self.G, opt, sp[:b // 2], gl[:b // 2], noises[0])
         sp_mix = swap(sp)
         L = {}
         l1 = (rec - real[:b // 2]).abs().mean()
@@ -409,7 +410,7 @@ class OracleModel:
             L["G_L1"] = l1 * opt.lambda_L1
         if opt.crop_size >= 1024:
             real, gl, sp_mix = real[b // 2:], gl[b // 2:], sp_mix[b // 2:]
-        mix = generator_forward(self.G, opt, sp_mix, gl)
+        mix = generator_forward(self.G, opt, sp_mix, gl, noises[1])
         if opt.lambda_GAN > 0:
             L["G_GAN_rec"] = gan_loss(discriminator_forward(self.D, opt, rec), True) * (opt.lambda_GAN * 0.5)
             L["G_GAN_mix"] = gan_loss(discriminator_forward(self.D, opt, mix), True) * (opt.lambda_GAN * 1.0)
