@@ -6,15 +6,19 @@
 // GEMM view: M = output pixels, N = output channels, K = taps x channels.  One CTA computes a
 // 128 (pixels) x BLOCK_N (channels) tile:
 //   * the 128 pixels are a (tn x th x tw) box of the NHWC output; for tap t the matching A tile is the SAME box of
-//     the input shifted by (oy_t, ox_t) — fetched with ONE 4-D TMA (box 32ch x tw x th x tn, element stride = conv
-//     stride), out-of-bounds rows/columns zero-filled by the TMA unit (that is the conv's zero padding), landing in
-//     shared memory directly in the K-major 128-byte-swizzled layout wgmma consumes: no im2col buffer, no
-//     register staging;
+//     the input shifted by (oy_t, ox_t), out-of-bounds rows/columns zero-filled by the TMA unit (that is the conv's zero
+//     padding), landing in shared memory directly in the K-major 128-byte-swizzled layout wgmma consumes: no im2col
+//     buffer, no register staging;
+//   * tap groups: taps with the same ox whose oy differ by stride * d read the same input rows d output rows apart, so
+//     they share ONE 4-D TMA box of th + span rows (box 32ch x tw x (th + span) x tn, element stride = conv stride) and
+//     each tap's A tile starts d * tw rows into it (a 3x3 stride-1 conv loads 3 boxes of th + 2 rows per channel block
+//     instead of 9 of th rows).  K runs (group, channel block, tap);
 //   * B tile = 32 (k) x BLOCK_N rows of the [Cout, taps*C] filter matrix, 2-D TMA, same swizzle;
 //   * warps 0..7 = two consumer warpgroups, each issuing m64 x BLOCK_N x k8 wgmma over its 64 tile rows; warp 8 = TMA
 //     producer (one lane);
-//   * STAGES-deep mbarrier ring (full/empty); a consumer warp releases a stage once the wgmma group that read it has
-//     retired (wgmma.wait_group 1 keeps the next group in flight);
+//   * two mbarrier rings (full/empty): A boxes and B tiles.  A consumer warp releases a B stage once the wgmma group that
+//     read it has retired (wgmma.wait_group 1 keeps the next group in flight), and an A box once the group of the last
+//     tap reading it has;
 //   * epilogue: accumulators -> the swizzled staging layout of the output tensor map (reusing the ring) -> bias / noise /
 //     leaky-ReLU / residual / TF32 rounding per 32-channel row piece -> TMA store, which also clips ragged tile edges.
 // fprop uses it with taps (r - pad_t, s - pad_l); dgrad with taps (pad_t - r, pad_l - s) over dy and the [C, R*S*K]
@@ -60,6 +64,7 @@ constexpr int TC_THREADS = 288;                // 2 consumer warpgroups + 1 prod
 constexpr int TC_CONSUMERS = 256;
 constexpr int TC_BK = 32;                      // fp32 elements per K block = one 128-byte swizzle row
 constexpr int TC_A_BYTES = 128 * TC_BK * 4;    // 16 KB
+constexpr int TC_BOX_PIXELS = 160;             // largest A box (th + span rows of tw pixels): 20 KB
 
 struct TcParams {
     int num_cblk;                 // source channels / 32
@@ -71,7 +76,11 @@ struct TcParams {
     int src_c;                    // source channels
     int o_mul, o_offy, o_offx;    // output sub-grid -> full-resolution pixel (strided outputs of transposed conv)
     int FH, FW;                   // full-resolution output extent (for noise / residual addressing)
-    short oy[TC_MAX_TAPS], ox[TC_MAX_TAPS];   // source pixel = stride * output pixel + (oy, ox)
+    int ngroups;                  // tap groups (tc_plan_groups)
+    int box_rows;                 // output rows per A box: th + the largest group span
+    short gy[TC_MAX_TAPS], gx[TC_MAX_TAPS];   // group g's box: source pixel = stride * output pixel + (gy, gx)
+    unsigned char g_end[TC_MAX_TAPS];         // group g holds taps [g_end[g - 1], g_end[g]) (taps in K order)
+    unsigned char a_row[TC_MAX_TAPS];         // first row of the tap's 128-row A tile inside its group's box (d * tw)
     int wk[TC_MAX_TAPS];          // K offset of the tap's filter slice inside a wmat row
     int w_nstride;                // filter rows between consecutive images (0 = one filter for the batch; Ncol = per-sample
                                   // filters [N, Ncol, Ktot], the style-modulated convolution, with tn == 1)
@@ -125,8 +134,9 @@ constexpr int tc_min_blocks() { return SPLIT && BLOCK_N >= 64 ? 1 : 2; }
 
 template <int BLOCK_N, bool SPLIT>
 constexpr size_t tc_smem_bytes() {
-    // stage ring (A + B, or A + B_hi + B_lo, per stage); the epilogue staging (BLOCK_N/32 chunks of 16 KB) reuses it after the
-    // main loop.
+    // A ring (STAGES x 16 KB: STAGES boxes of th rows, or at least two of up to TC_BOX_PIXELS rows) + B ring (STAGES x B, or
+    // B_hi + B_lo); the epilogue staging (BLOCK_N/32 chunks of 16 KB) reuses it after the main loop.
+    static_assert(tc_stages<BLOCK_N, SPLIT>() * TC_A_BYTES >= 2 * TC_BOX_PIXELS * 128, "the A ring must hold two boxes");
     size_t ring = (size_t)tc_stages<BLOCK_N, SPLIT>() * (TC_A_BYTES + (SPLIT ? 2 : 1) * BLOCK_N * 128);
     size_t epi = (size_t)(BLOCK_N / 32) * TC_A_BYTES;
     return (ring > epi ? ring : epi) + 1024 /*alignment slack*/ + 256 /*barriers*/;
@@ -162,17 +172,21 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
     const CUtensorMap& map_w = batch.w;
     constexpr int STAGES = tc_stages<BLOCK_N, SPLIT>();
     constexpr int B_BYTES = BLOCK_N * 128;
-    constexpr int STAGE_BYTES = TC_A_BYTES + (SPLIT ? 2 : 1) * B_BYTES;
+    constexpr int B_STAGE = (SPLIT ? 2 : 1) * B_BYTES;
     constexpr int NCHUNK = BLOCK_N / 32;
     constexpr int NACC = BLOCK_N / 2;                                   // fp32 accumulators per thread (m64 x BLOCK_N / 128)
 
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;       // SWIZZLE_128B needs 1024-byte alignment
-    constexpr uint32_t RING = (uint32_t)STAGES * STAGE_BYTES;
+    // A ring [0, A_RING): as many boxes as fit (STAGES of th rows, fewer of th + span rows); B ring: STAGES tiles after it
+    constexpr uint32_t A_RING = (uint32_t)STAGES * TC_A_BYTES;
+    constexpr uint32_t RING = A_RING + (uint32_t)STAGES * B_STAGE;
     constexpr uint32_t EPI = (uint32_t)NCHUNK * TC_A_BYTES;
     constexpr uint32_t BAR_OFF = RING > EPI ? RING : EPI;
-    const uint32_t bar_full = base + BAR_OFF;                          // STAGES x 8 bytes
-    const uint32_t bar_empty = bar_full + 8 * STAGES;
+    const uint32_t a_full = base + BAR_OFF;                            // STAGES x 8 bytes each
+    const uint32_t a_empty = a_full + 8 * STAGES;
+    const uint32_t b_full = a_empty + 8 * STAGES;
+    const uint32_t b_empty = b_full + 8 * STAGES;
     uint8_t* smem_gen = smem_raw + (base - smem_u32(smem_raw));       // generic pointer to the aligned base
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -184,7 +198,8 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
     const int tnb = tile;
     const int q0 = tq * p.tw, p0 = tp * p.th, n0 = tnb * p.tn;
     const int col0 = blockIdx.y * BLOCK_N;
-    const int KB = p.ntaps * p.num_cblk;
+    const uint32_t a_bytes = (uint32_t)(p.box_rows * p.tw * p.tn * 128);   // a multiple of 1024 (tc_plan_groups)
+    const int a_slots = (int)(A_RING / a_bytes);                          // >= 2
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_src) : "memory");
@@ -192,27 +207,38 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
         if constexpr (SPLIT) asm volatile("prefetch.tensormap [%0];" ::"l"(&batch.w_lo) : "memory");
         for (int s = 0; s < STAGES; ++s) {
-            mbar_init(bar_full + 8 * s, 1);
-            mbar_init(bar_empty + 8 * s, TC_CONSUMERS / 32);          // one arrival per consumer warp
+            mbar_init(a_full + 8 * s, 1);
+            mbar_init(a_empty + 8 * s, TC_CONSUMERS / 32);            // one arrival per consumer warp
+            mbar_init(b_full + 8 * s, 1);
+            mbar_init(b_empty + 8 * s, TC_CONSUMERS / 32);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
     if (warp == TC_CONSUMERS / 32) {
-        // ===================================================== TMA producer
+        // ===================================================== TMA producer: one A box per (group, channel block), one B
+        // tile per (channel block, tap), in the consumers' order
         if (lane == 0) {
             const int wrow = col0 + n0 * p.w_nstride;
-            for (int kb = 0; kb < KB; ++kb) {
-                const int s = kb % STAGES;
-                const uint32_t ph = (uint32_t)(kb / STAGES) & 1u;
-                mbar_wait(bar_empty + 8 * s, ph ^ 1u);
-                const int t = kb / p.num_cblk, cb = kb - t * p.num_cblk;
-                const uint32_t sa = base + (uint32_t)s * STAGE_BYTES, sb = sa + TC_A_BYTES;
-                mbar_expect_tx(bar_full + 8 * s, STAGE_BYTES);
-                tma_load_4d(sa, &map_src, bar_full + 8 * s, cb * TC_BK, q0 * p.stride + p.ox[t], p0 * p.stride + p.oy[t], n0);
-                tma_load_2d(sb, &map_w, bar_full + 8 * s, p.wk[t] + cb * TC_BK, wrow);
-                if constexpr (SPLIT) tma_load_2d(sb + B_BYTES, &batch.w_lo, bar_full + 8 * s, p.wk[t] + cb * TC_BK, wrow);
+            int kb = 0, as = 0;
+            uint32_t aph = 0;
+            for (int g = 0, t0 = 0; g < p.ngroups; t0 = p.g_end[g++]) {
+                for (int cb = 0; cb < p.num_cblk; ++cb) {
+                    mbar_wait(a_empty + 8 * as, aph ^ 1u);
+                    mbar_expect_tx(a_full + 8 * as, a_bytes);
+                    tma_load_4d(base + (uint32_t)as * a_bytes, &map_src, a_full + 8 * as, cb * TC_BK, q0 * p.stride + p.gx[g],
+                                p0 * p.stride + p.gy[g], n0);
+                    if (++as == a_slots) { as = 0; aph ^= 1u; }
+                    for (int t = t0; t < p.g_end[g]; ++t, ++kb) {
+                        const int s = kb % STAGES;
+                        mbar_wait(b_empty + 8 * s, ((uint32_t)(kb / STAGES) & 1u) ^ 1u);
+                        const uint32_t sb = base + A_RING + (uint32_t)s * B_STAGE;
+                        mbar_expect_tx(b_full + 8 * s, B_STAGE);
+                        tma_load_2d(sb, &map_w, b_full + 8 * s, p.wk[t] + cb * TC_BK, wrow);
+                        if constexpr (SPLIT) tma_load_2d(sb + B_BYTES, &batch.w_lo, b_full + 8 * s, p.wk[t] + cb * TC_BK, wrow);
+                    }
+                }
             }
         }
         return;
@@ -224,54 +250,73 @@ conv_wg_kernel(const __grid_constant__ TcBatch batch) {
     float part[SPLIT ? NACC : 1];                                      // split-TF32: the current stage's sums
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < KB; ++kb) {
-        const int s = kb % STAGES;
-        mbar_wait(bar_full + 8 * s, (uint32_t)(kb / STAGES) & 1u);
-        const uint32_t sa = base + (uint32_t)s * STAGE_BYTES, sb = sa + TC_A_BYTES;
-        if constexpr (SPLIT) {
-            // A fragments (m16 x k8 per warp, k steps k = 0..3) out of the swizzled stage: rows r = 64 wg + 16 (warp & 3) +
-            // lane / 4 (+ 8), columns 8 k + lane % 4 (+ 4).  r & 7 == lane / 4, so the 16-byte piece (2 k or 2 k + 1) ^ (lane / 4)
-            // and the word lane % 4 put the warp's 32 loads on 32 distinct banks.
-            const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-            const float* arow = reinterpret_cast<const float*>(smem_gen + (sa - base) + (uint32_t)r * 128) + (lane & 3);
-            uint32_t ahi[TC_BK / 8][4], alo[TC_BK / 8][4];
+    int kb = 0, as = 0, a_done = -1;                                   // a_done: A slot whose last wgmma group is in flight
+    uint32_t aph = 0;
+    for (int g = 0, t0 = 0; g < p.ngroups; t0 = p.g_end[g++]) {
+        for (int cb = 0; cb < p.num_cblk; ++cb) {
+            mbar_wait(a_full + 8 * as, aph);
+            const uint32_t sbox = base + (uint32_t)as * a_bytes;
+            for (int t = t0; t < p.g_end[g]; ++t, ++kb) {
+                const int s = kb % STAGES;
+                mbar_wait(b_full + 8 * s, (uint32_t)(kb / STAGES) & 1u);
+                // the tap's A tile starts a_row rows into the box: a multiple of 8 rows = 1024 bytes, so the swizzle phase
+                // (row & 7) and the descriptor's atom alignment are those of the box
+                const uint32_t sa = sbox + (uint32_t)p.a_row[t] * 128, sb = base + A_RING + (uint32_t)s * B_STAGE;
+                if constexpr (SPLIT) {
+                    // A fragments (m16 x k8 per warp, k steps k = 0..3) out of the swizzled tile: rows r = 64 wg + 16 (warp & 3) +
+                    // lane / 4 (+ 8), columns 8 k + lane % 4 (+ 4).  r & 7 == lane / 4, so the 16-byte piece (2 k or 2 k + 1) ^ (lane / 4)
+                    // and the word lane % 4 put the warp's 32 loads on 32 distinct banks.
+                    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+                    const float* arow = reinterpret_cast<const float*>(smem_gen + (sa - base) + (uint32_t)r * 128) + (lane & 3);
+                    uint32_t ahi[TC_BK / 8][4], alo[TC_BK / 8][4];
 #pragma unroll
-            for (int k = 0; k < TC_BK / 8; ++k) {
-                const int p0 = ((2 * k) ^ (lane >> 2)) * 4, p1 = ((2 * k + 1) ^ (lane >> 2)) * 4;
-                split_tf32(arow[p0], ahi[k][0], alo[k][0]);
-                split_tf32(arow[8 * 32 + p0], ahi[k][1], alo[k][1]);
-                split_tf32(arow[p1], ahi[k][2], alo[k][2]);
-                split_tf32(arow[8 * 32 + p1], ahi[k][3], alo[k][3]);
+                    for (int k = 0; k < TC_BK / 8; ++k) {
+                        const int p0 = ((2 * k) ^ (lane >> 2)) * 4, p1 = ((2 * k + 1) ^ (lane >> 2)) * 4;
+                        split_tf32(arow[p0], ahi[k][0], alo[k][0]);
+                        split_tf32(arow[8 * 32 + p0], ahi[k][1], alo[k][1]);
+                        split_tf32(arow[p1], ahi[k][2], alo[k][2]);
+                        split_tf32(arow[8 * 32 + p1], ahi[k][3], alo[k][3]);
+                    }
+                    const uint64_t db = make_wgmma_desc_sw128(sb), dbl = make_wgmma_desc_sw128(sb + B_BYTES);
+                    wgmma_fence();
+                    Wgmma<BLOCK_N>::template mma_rs<0>(part, alo[0], db);
+                    Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[0], dbl);
+                    Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[0], db);
+#pragma unroll
+                    for (int k = 1; k < TC_BK / 8; ++k) {
+                        Wgmma<BLOCK_N>::template mma_rs<1>(part, alo[k], db + (uint64_t)(k * 2));
+                        Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[k], dbl + (uint64_t)(k * 2));
+                        Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[k], db + (uint64_t)(k * 2));
+                    }
+                } else {
+                    const uint64_t da = make_wgmma_desc_sw128(sa + (uint32_t)wg * (64 * 128)), db = make_wgmma_desc_sw128(sb);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < TC_BK / 8; ++k) {
+                        // advance 8 tf32 = 32 bytes along K inside the swizzle atom: +2 in the (addr >> 4) field
+                        Wgmma<BLOCK_N>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
+                    }
+                }
+                wgmma_commit();
+                if constexpr (SPLIT) {
+                    wgmma_wait<0>();       // the next stage's A fragments reuse these registers: retire this group before loading them
+                    if (lane == 0) {
+                        mbar_arrive(b_empty + 8 * s);
+                        if (t + 1 == p.g_end[g]) mbar_arrive(a_empty + 8 * as);
+                    }
+#pragma unroll
+                    for (int i = 0; i < NACC; ++i) acc[i] += part[i];
+                } else {
+                    wgmma_wait<1>();                                   // the group of B stage kb - 1 has retired
+                    if (lane == 0) {
+                        if (kb > 0) mbar_arrive(b_empty + 8 * ((kb - 1) % STAGES));
+                        if (a_done >= 0) mbar_arrive(a_empty + 8 * a_done);
+                    }
+                    a_done = -1;
+                }
             }
-            const uint64_t db = make_wgmma_desc_sw128(sb), dbl = make_wgmma_desc_sw128(sb + B_BYTES);
-            wgmma_fence();
-            Wgmma<BLOCK_N>::template mma_rs<0>(part, alo[0], db);
-            Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[0], dbl);
-            Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[0], db);
-#pragma unroll
-            for (int k = 1; k < TC_BK / 8; ++k) {
-                Wgmma<BLOCK_N>::template mma_rs<1>(part, alo[k], db + (uint64_t)(k * 2));
-                Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[k], dbl + (uint64_t)(k * 2));
-                Wgmma<BLOCK_N>::template mma_rs<1>(part, ahi[k], db + (uint64_t)(k * 2));
-            }
-        } else {
-            const uint64_t da = make_wgmma_desc_sw128(sa + (uint32_t)wg * (64 * 128)), db = make_wgmma_desc_sw128(sb);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < TC_BK / 8; ++k) {
-                // advance 8 tf32 = 32 bytes along K inside the swizzle atom: +2 in the (addr >> 4) field
-                Wgmma<BLOCK_N>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2));
-            }
-        }
-        wgmma_commit();
-        if constexpr (SPLIT) {
-            wgmma_wait<0>();       // the next stage's A fragments reuse these registers: retire this group before loading them
-            if (lane == 0) mbar_arrive(bar_empty + 8 * s);
-#pragma unroll
-            for (int i = 0; i < NACC; ++i) acc[i] += part[i];
-        } else {
-            wgmma_wait<1>();                                           // the group of stage kb - 1 has retired
-            if (kb > 0 && lane == 0) mbar_arrive(bar_empty + 8 * ((kb - 1) % STAGES));
+            if constexpr (!SPLIT) a_done = as;                         // released once the group of its last tap retires
+            if (++as == a_slots) { as = 0; aph ^= 1u; }
         }
     }
     wgmma_wait<0>();
@@ -356,6 +401,47 @@ static bool tc_shape_ok(int src_c, int ncol, int ntaps, int stride, int ow) {
     return true;
 }
 
+static int floor_mod(int a, int m) { return ((a % m) + m) % m; }
+
+// Tap groups.  Source pixel = stride * output pixel + (oy, ox), so two taps with the same ox whose oy differ by stride * d
+// read the same input box d output rows apart: they share one A box that starts at the group's smallest oy, and tap t's
+// 128-row tile starts a_row[t] = d * tw rows into it.  That start must stay on a 1024-byte swizzle atom (8 rows), which holds
+// for one-image tiles (tn == 1) of width 8 or 16; any other tile puts every tap in a group of its own, a box of th rows.
+// A group spans at most TC_BOX_PIXELS / tw - th rows (a longer column splits).  The tensor map fixes one box height for the
+// problem, th + the largest span, so a group of smaller span loads rows it does not read (stride 2: one in th + 1).
+// Taps are ordered by (ox, oy mod stride, oy), which makes each group a contiguous run of the K order.
+static void tc_plan_groups(const TcProblem& pr, TcParams& p) {
+    const int st = pr.stride;
+    const int max_span = p.tn == 1 && (p.tw == 8 || p.tw == 16) ? TC_BOX_PIXELS / p.tw - p.th : 0;
+    auto before = [&](int a, int b) {
+        if (pr.ox[a] != pr.ox[b]) return pr.ox[a] < pr.ox[b];
+        const int ma = floor_mod(pr.oy[a], st), mb = floor_mod(pr.oy[b], st);
+        return ma != mb ? ma < mb : pr.oy[a] < pr.oy[b];
+    };
+    int order[TC_MAX_TAPS];
+    for (int t = 0; t < pr.ntaps; ++t) {
+        int j = t;
+        for (; j > 0 && before(t, order[j - 1]); --j) order[j] = order[j - 1];
+        order[j] = t;
+    }
+    int span = 0;
+    p.ngroups = 0;
+    for (int i = 0; i < pr.ntaps; ++i) {
+        const int t = order[i], g = p.ngroups - 1;
+        if (g < 0 || pr.ox[t] != p.gx[g] || floor_mod(pr.oy[t] - p.gy[g], st) != 0 || (pr.oy[t] - p.gy[g]) / st > max_span) {
+            p.gy[p.ngroups] = (short)pr.oy[t];
+            p.gx[p.ngroups] = (short)pr.ox[t];
+            ++p.ngroups;
+        }
+        const int d = (pr.oy[t] - p.gy[p.ngroups - 1]) / st;
+        if (d > span) span = d;
+        p.a_row[i] = (unsigned char)(d * p.tw);
+        p.wk[i] = pr.wk[t];
+        p.g_end[p.ngroups - 1] = (unsigned char)(i + 1);
+    }
+    p.box_rows = p.th + span;
+}
+
 static void tc_fill_params(const TcProblem& pr, const EpiParams& e, TcParams& p) {
     p.num_cblk = pr.SC / 32;
     p.ntaps = pr.ntaps;
@@ -365,7 +451,7 @@ static void tc_fill_params(const TcProblem& pr, const EpiParams& e, TcParams& p)
     p.tiles_h = (pr.OH + p.th - 1) / p.th;
     p.tiles_n = (pr.SN + p.tn - 1) / p.tn;
     p.ON = pr.SN; p.OH = pr.OH; p.OW = pr.OW; p.Ncol = pr.Ncol; p.src_c = pr.SC;
-    for (int t = 0; t < pr.ntaps; ++t) { p.oy[t] = (short)pr.oy[t]; p.ox[t] = (short)pr.ox[t]; p.wk[t] = pr.wk[t]; }
+    tc_plan_groups(pr, p);
     p.o_mul = pr.o_mul; p.o_offy = pr.o_offy; p.o_offx = pr.o_offx; p.FH = pr.FH; p.FW = pr.FW;
     p.w_nstride = pr.w_per_sample ? pr.Ncol : 0;
     p.epi = e;
@@ -389,7 +475,7 @@ int encode_act_map(CUtensorMap* m, const float* ptr, int N, int H, int W, int C,
 
 static int tc_encode_maps(const TcProblem& pr, const TcParams& p, int b_rows, CUtensorMap* msrc, CUtensorMap* mw, CUtensorMap* mout) {
     {
-        int rc = encode_act_map(msrc, pr.src, pr.SN, pr.SH, pr.SW, pr.SC, p.tw, p.th, p.tn, pr.stride);
+        int rc = encode_act_map(msrc, pr.src, pr.SN, pr.SH, pr.SW, pr.SC, p.tw, p.box_rows, p.tn, pr.stride);
         if (rc) return rc;
     }
     {
