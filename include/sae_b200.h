@@ -31,7 +31,7 @@ extern "C" {
 #define SAE_E_UNSUPPORTED  -3   /* valid request this build has no kernel for                */
 
 /* ABI version of this header; bumped on any signature change. */
-#define SAE_ABI_VERSION 15
+#define SAE_ABI_VERSION 16
 int         sae_abi_version(void);
 const char* sae_last_error(void);
 /* number of kernels launched by this library in the calling process since load
@@ -311,6 +311,22 @@ int sae_conv2d_wgrad_modulated_3xtf32(const float* dy, const float* x, const flo
 int sae_adam_step(float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets, const int64_t* sizes, int n,
                   float* exp_avg, float* exp_avg_sq, float* steps, float lr, float beta1, float beta2, float eps,
                   float grad_scale, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Skip-on-non-finite guard of the optimizer step (ABI 16; SwappingAutoencoderOptimizer with opt.skip_nonfinite_steps).
+ * sae_nonfinite_count: counts the non-finite elements (NaN, +Inf, -Inf) of n fp32 tensors.  ptrs / sizes: device arrays of
+ *   n pointers / n int64 element counts; a NULL pointer skips its tensor.  counts: device array of n + 1 entries that the
+ *   caller zero-fills, as the dw of sae_conv2d_wgrad; the scan ADDS tensor t's count to counts[t] and the sum of all to
+ *   counts[n].  +-FLT_MAX, denormals and -0.0 are finite.  Any pointer alignment and size (64-bit indexing); integer sums,
+ *   so the result is exact and independent of the schedule (deterministic mode needs no twin).  n <= 65535.
+ * sae_adam_step_guarded: sae_adam_step, except that the update is dropped on the device when *skip != 0 (read by the
+ *   kernels, never by the host): parameters, exp_avg, exp_avg_sq and steps are left bitwise unchanged.  skip normally
+ *   points at counts[n] of a sae_nonfinite_count over the same g_ptrs, issued earlier on the same stream.
+ * ------------------------------------------------------------------------------------------ */
+int sae_nonfinite_count(const float* const* ptrs, const int64_t* sizes, int n, unsigned long long* counts, void* stream);
+int sae_adam_step_guarded(float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets, const int64_t* sizes,
+                          int n, float* exp_avg, float* exp_avg_sq, float* steps, float lr, float beta1, float beta2,
+                          float eps, float grad_scale, const unsigned long long* skip, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Random-crop resampler of the patch discriminator (SURVEY.md §8 f1).  Replaces

@@ -69,6 +69,12 @@ def _need_cuda(*ts, strided=False):
             raise _lib.SaeError("sae_b200 kernels need contiguous NHWC storage")
 
 
+def _need_int64(t):
+    """the 64-bit integer counters of the non-finite guard (unsigned long long in the C ABI)"""
+    if not t.is_cuda or t.dtype != torch.int64 or not t.is_contiguous():
+        raise _lib.SaeError("non-finite guard counters must be contiguous int64 CUDA tensors")
+
+
 class PointerTables:
     """Device copies of host address lists (tuples of ``data_ptr()``), cached by content.  The pinned staging rows are
     allocated up front — a miss costs a device allocation and an async copy, so a miss inside a CUDA-graph capture is legal:
@@ -553,22 +559,42 @@ class CudaKernels:
 
 
     # ----------------------------------------------------------------- Adam
-    def adam_step(self, params, grads, offsets, sizes, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, grad_scale, cache):
+    def adam_step(self, params, grads, offsets, sizes, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, grad_scale, cache,
+                  skip=None):
         """One multi-tensor Adam update (torch.optim.Adam semantics) of ``params`` (list of tensors).  grads: list aligned with
         params — a tensor (the parameter's own gradient, or a view into the flat all-reduce bucket) or None (parameter
         skipped, its step count untouched).  offsets / sizes: device int64 tensors locating each parameter's moments in
         the flat ``exp_avg`` / ``exp_avg_sq``; steps: device float tensor, one count per parameter.  cache: the caller's
-        ``PointerTables`` (device copies of the address lists)."""
+        ``PointerTables`` (device copies of the address lists).  skip: optional one-element device int64 tensor (the total of
+        ``nonfinite_count``); the kernels drop the whole update when it is non-zero (sae_adam_step_guarded)."""
         dev = exp_avg.device
         p_tab = cache.get(tuple(p.data_ptr() for p in params))
         g_tab = cache.get(tuple(0 if g is None else g.data_ptr() for g in grads))
         for g in grads:
             if g is not None and (not g.is_cuda or g.dtype != torch.float32 or not g.is_contiguous()):
                 raise _lib.SaeError("adam_step: gradients must be contiguous fp32 CUDA tensors")
+        args = (_ptr(p_tab), _ptr(g_tab), _ptr(offsets), _ptr(sizes), len(params), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(steps), lr,
+                beta1, beta2, eps, grad_scale)
         with torch.cuda.device(dev):
-            check(self.lib.sae_adam_step(_ptr(p_tab), _ptr(g_tab), _ptr(offsets), _ptr(sizes), len(params), _ptr(exp_avg),
-                                         _ptr(exp_avg_sq), _ptr(steps), lr, beta1, beta2, eps, grad_scale, _stream()),
-                  "sae_adam_step")
+            if skip is None:
+                check(self.lib.sae_adam_step(*args, _stream()), "sae_adam_step")
+            else:
+                _need_int64(skip)
+                check(self.lib.sae_adam_step_guarded(*args, _ptr(skip), _stream()), "sae_adam_step_guarded")
+
+    def nonfinite_count(self, tensors, sizes, counts, cache):
+        """counts[i] += number of NaN / +-Inf elements of tensors[i] (None: skipped), counts[n] += their sum; one launch.
+        tensors: contiguous fp32 CUDA tensors; sizes: device int64 tensor of their element counts (the parameters' sizes);
+        counts: device int64 tensor of n + 1 entries, zero-filled by the caller; cache: ``PointerTables``."""
+        _need_int64(counts)
+        for t in tensors:
+            _need_cuda(t)
+        if counts.numel() != len(tensors) + 1 or sizes.numel() != len(tensors):
+            raise _lib.SaeError("nonfinite_count: counts needs n + 1 entries and sizes n")
+        tab = cache.get(tuple(0 if t is None else t.data_ptr() for t in tensors))
+        with torch.cuda.device(counts.device):
+            check(self.lib.sae_nonfinite_count(_ptr(tab), _ptr(sizes), len(tensors), _ptr(counts), _stream()),
+                  "sae_nonfinite_count")
 
     # ----------------------------------------------------------------- ToRGB
     def torgb_forward(self, x, s, w, bias, wscale):

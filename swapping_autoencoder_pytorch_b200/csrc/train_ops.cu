@@ -14,10 +14,14 @@ namespace sae {
 //   t <- t + 1;  m <- m + (1 - b1)(g - m);  v <- b2 v + (1 - b2) g^2;
 //   p <- p - lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps)
 // A tensor whose gradient pointer is null is skipped and keeps its step count, like a parameter whose .grad is None.
+// skip (optional, read on the device): when it points at a non-zero count the whole update is dropped — both kernels return
+// before touching anything (sae_adam_step_guarded after sae_nonfinite_count).
 __global__ void __launch_bounds__(256)
 adam_kernel(float* const* __restrict__ p_ptrs, const float* const* __restrict__ g_ptrs, const int64_t* __restrict__ offsets,
             const int64_t* __restrict__ sizes, float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
-            const float* __restrict__ steps, float lr, float b1, float b2, float eps, float gscale) {
+            const float* __restrict__ steps, float lr, float b1, float b2, float eps, float gscale,
+            const unsigned long long* __restrict__ skip) {
+    if (skip && *skip) return;
     const int t = blockIdx.y;
     const float* g = g_ptrs[t];
     if (g == nullptr) return;
@@ -59,7 +63,9 @@ adam_kernel(float* const* __restrict__ p_ptrs, const float* const* __restrict__ 
     }
 }
 
-__global__ void adam_advance_kernel(const float* const* __restrict__ g_ptrs, float* __restrict__ steps, int n) {
+__global__ void adam_advance_kernel(const float* const* __restrict__ g_ptrs, float* __restrict__ steps, int n,
+                                    const unsigned long long* __restrict__ skip) {
+    if (skip && *skip) return;
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n && g_ptrs[i] != nullptr) steps[i] += 1.f;
 }
@@ -213,9 +219,9 @@ static inline unsigned grid_1d(int64_t work, int threads, int per_sm) {
 
 using namespace sae;
 
-extern "C" int sae_adam_step(float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets, const int64_t* sizes,
-                             int n, float* exp_avg, float* exp_avg_sq, float* steps, float lr, float beta1, float beta2,
-                             float eps, float grad_scale, void* stream) {
+static int adam_launch(float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets, const int64_t* sizes, int n,
+                       float* exp_avg, float* exp_avg_sq, float* steps, float lr, float beta1, float beta2, float eps,
+                       float grad_scale, const unsigned long long* skip, void* stream) {
     if (n == 0) return SAE_OK;
     if (!p_ptrs || !g_ptrs || !offsets || !sizes || !exp_avg || !exp_avg_sq || !steps || n < 0)
         return fail(SAE_E_INVALID, "adam_step: bad arguments");
@@ -223,11 +229,28 @@ extern "C" int sae_adam_step(float* const* p_ptrs, const float* const* g_ptrs, c
         return fail(SAE_E_INVALID, "adam_step: betas must lie in [0, 1) and eps must be >= 0");
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid(48, (unsigned)n);
-    adam_kernel<<<grid, 256, 0, st>>>(p_ptrs, g_ptrs, offsets, sizes, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, grad_scale);
+    adam_kernel<<<grid, 256, 0, st>>>(p_ptrs, g_ptrs, offsets, sizes, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, grad_scale,
+                                      skip);
     int rc = check_launch("adam_step");
     if (rc) return rc;
-    adam_advance_kernel<<<(n + 255) / 256, 256, 0, st>>>(g_ptrs, steps, n);
+    adam_advance_kernel<<<(n + 255) / 256, 256, 0, st>>>(g_ptrs, steps, n, skip);
     return check_launch("adam_advance");
+}
+
+extern "C" int sae_adam_step(float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets, const int64_t* sizes,
+                             int n, float* exp_avg, float* exp_avg_sq, float* steps, float lr, float beta1, float beta2,
+                             float eps, float grad_scale, void* stream) {
+    return adam_launch(p_ptrs, g_ptrs, offsets, sizes, n, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, grad_scale, nullptr,
+                       stream);
+}
+
+extern "C" int sae_adam_step_guarded(float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets,
+                                     const int64_t* sizes, int n, float* exp_avg, float* exp_avg_sq, float* steps, float lr,
+                                     float beta1, float beta2, float eps, float grad_scale, const unsigned long long* skip,
+                                     void* stream) {
+    if (!skip && n != 0) return fail(SAE_E_INVALID, "adam_step_guarded: null skip pointer");
+    return adam_launch(p_ptrs, g_ptrs, offsets, sizes, n, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, grad_scale, skip,
+                       stream);
 }
 
 static int crop_params(CropParams& p, const float* flip, const float* scale, const float* offset, int Q, int num_crops, int C,

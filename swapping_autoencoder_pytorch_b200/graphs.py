@@ -30,7 +30,8 @@ class HalfStepGraphs:
         self.trainer = trainer
         self.warmup = warmup
         self.calls = {}
-        self.captured = {}        # (kind, input shape, kernel precision, deterministic) -> (graph, static_input, static_outputs, launches)
+        # (kind, input shape, kernel precision, deterministic, non-finite guard) -> (graph, static_input, static_outputs, launches, ...)
+        self.captured = {}
         self.pool = None
         self.stream = None             # side stream shared by the eager warm-up calls and every capture (see _side)
         self.disabled = None
@@ -58,7 +59,7 @@ class HalfStepGraphs:
 
     def _tail(self, kind):
         """world > 1: pack the static gradient buffers, all-reduce, Adam reading the bucket (optimizer.exchange_and_step)"""
-        self.trainer.exchange_and_step(self._optimizer(kind), self._params(kind))
+        self.trainer.exchange_and_step(self._optimizer(kind), self._params(kind), kind=kind)
 
     def _side(self, fn):
         """Run ``fn`` on the capture stream.  The warm-up calls must run where the capture will: autograd remembers
@@ -98,13 +99,15 @@ class HalfStepGraphs:
             return body(images)
         # a graph records the kernels of one precision mode (backend.CudaKernels.precision): switching the mode captures new
         # graphs, after warm-up calls of their own (the other mode's kernels initialise lazily, outside any capture).  The same
-        # holds for the deterministic mode (backend.CudaKernels.deterministic_mode()), which records other kernels.
+        # holds for the deterministic mode (backend.CudaKernels.deterministic_mode()), which records other kernels, and for the
+        # non-finite guard (opt.skip_nonfinite_steps), which adds the scan and the guarded update.
         k = backend.kernels()
         precision = getattr(k, "precision", "tf32")
         det = bool(getattr(k, "deterministic_mode", lambda: False)())
-        n = self.calls.get((kind, precision, det), 0)
-        self.calls[(kind, precision, det)] = n + 1
-        key = (kind, tuple(images.shape), precision, det)
+        guard = self.trainer.nonfinite_guard_on()
+        n = self.calls.get((kind, precision, det, guard), 0)
+        self.calls[(kind, precision, det, guard)] = n + 1
+        key = (kind, tuple(images.shape), precision, det, guard)
         hit = self.captured.get(key)
         if hit is None:
             if n < self.warmup:
@@ -190,6 +193,8 @@ class HalfStepGraphs:
             static_in.copy_(images)
         for p in self._params(kind):
             p.grad = None                    # gradients of the eager calls: the capture allocates its own static set
+        if key[4]:
+            self.trainer.nonfinite_guard(kind)          # its counters must live outside the graph's pool
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
         if self.stream is None:

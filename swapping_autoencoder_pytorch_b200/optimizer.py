@@ -53,7 +53,9 @@ class MultiTensorAdam:
                 p.grad.detach_().zero_()
 
     @torch.no_grad()
-    def step(self, grads=None, grad_scale=1.0):
+    def step(self, grads=None, grad_scale=1.0, guard=None):
+        """guard: a ``NonfiniteGuard`` — scan the gradients this update reads and drop the update on the device when any
+        element is not finite (opt.skip_nonfinite_steps)"""
         st = self._state()
         g = self.param_groups[0]
         if grads is None:
@@ -64,8 +66,9 @@ class MultiTensorAdam:
         params = self.params
         if st.exp_avg.dtype != params[0].dtype:           # fp64 runs of the CPU test-suite
             st.exp_avg, st.exp_avg_sq = st.exp_avg.to(params[0].dtype), st.exp_avg_sq.to(params[0].dtype)
+        kw = {} if guard is None else {"skip": guard.scan(grads, st.sizes_t, self._cache)}
         backend.kernels().adam_step(params, grads, st.offsets_t, st.sizes_t, st.exp_avg, st.exp_avg_sq, st.steps, g["lr"],
-                                    g["betas"][0], g["betas"][1], g["eps"], float(grad_scale), self._cache)
+                                    g["betas"][0], g["betas"][1], g["eps"], float(grad_scale), self._cache, **kw)
 
     # torch.optim.Adam's on-disk format, so optimizer checkpoints interoperate with the stock optimizer
     def state_dict(self):
@@ -96,6 +99,31 @@ class MultiTensorAdam:
             st.exp_avg[o:o + n].copy_(entry["exp_avg"].reshape(-1))
             st.exp_avg_sq[o:o + n].copy_(entry["exp_avg_sq"].reshape(-1))
             st.steps[i] = float(entry["step"])
+
+
+class NonfiniteGuard:
+    """Device state of the skip-on-non-finite guard for one kind of half-step (D, R1 or G).  ``scan`` counts the non-finite
+    elements of the gradients Adam is about to read (one kernel) and returns the total as the ``skip`` argument of the
+    guarded update; it also advances this kind's skip counter and, when the total is non-zero, keeps the per-tensor counts
+    as the report.  All of it stays on the device, so it is capturable and costs no host sync."""
+
+    def __init__(self, n, skipped):
+        dev = skipped.device
+        self.counts = torch.zeros(n + 1, dtype=torch.int64, device=dev)     # the latest scan: per tensor, then the total
+        self.report = torch.zeros(n, dtype=torch.int64, device=dev)         # the latest scan with a non-zero total
+        self.skipped = skipped                                              # one-element view of the trainer's counters
+
+    def scan(self, grads, sizes, cache):
+        self.counts.zero_()
+        backend.kernels().nonfinite_count(grads, sizes, self.counts, cache)
+        total = self.counts[-1:]
+        bad = total != 0
+        self.skipped.add_(bad)
+        torch.where(bad, self.counts[:-1], self.report, out=self.report)
+        return total
+
+
+NONFINITE_KINDS = ("D", "R1", "G")
 
 
 class SwappingAutoencoderOptimizer:
@@ -131,13 +159,57 @@ class SwappingAutoencoderOptimizer:
         # lazy regularisation correction of lr and betas (StyleGAN2 appendix B; reference :38-42)
         c = opt.R1_once_every / (1 + opt.R1_once_every)
         self.optimizer_D = MultiTensorAdam(self.Dparams, lr=opt.lr * c, betas=(opt.beta1 ** c, opt.beta2 ** c))
+        # skip-on-non-finite guard (extension, ``opt.skip_nonfinite_steps``): created on first use
+        self._nonfinite_skipped = None      # device int64 [3]: skipped half-steps per kind, NONFINITE_KINDS order
+        self._nonfinite_guards = {}
 
-    def exchange_and_step(self, optimizer, params):
-        """optimizer step of one half-step; with more than one rank: pack -> all-reduce (SUM) -> Adam reading the bucket"""
+    def nonfinite_guard_on(self):
+        return bool(getattr(self.opt, "skip_nonfinite_steps", False))
+
+    def _nonfinite_counters(self):
+        if self._nonfinite_skipped is None:
+            self._nonfinite_skipped = torch.zeros(len(NONFINITE_KINDS), dtype=torch.int64, device=self.Gparams[0].device)
+        return self._nonfinite_skipped
+
+    def nonfinite_guard(self, kind):
+        """the ``NonfiniteGuard`` of one kind of half-step ("D", "R1" or "G"), created on first use"""
+        g = self._nonfinite_guards.get(kind)
+        if g is None:
+            i = NONFINITE_KINDS.index(kind)
+            g = NonfiniteGuard(len(self.Gparams if kind == "G" else self.Dparams), self._nonfinite_counters()[i:i + 1])
+            self._nonfinite_guards[kind] = g
+        return g
+
+    def nonfinite_steps(self):
+        """{"D": n, "R1": n, "G": n}: half-steps of each kind whose update the guard dropped since construction (or as
+        restored by ``load_state_dict``); one device-to-host read"""
+        if self._nonfinite_skipped is None:
+            return {k: 0 for k in NONFINITE_KINDS}
+        return dict(zip(NONFINITE_KINDS, self._nonfinite_skipped.tolist()))
+
+    def nonfinite_report(self, kind):
+        """{state_dict key: non-finite element count} of the gradients of the most recent ``kind`` half-step that had any
+        ({} if none had); one device-to-host read"""
+        g = self._nonfinite_guards.get(kind)
+        if g is None:
+            if kind not in NONFINITE_KINDS:
+                raise ValueError(kind)
+            return {}
+        inner = getattr(self.model, "singlegpu_model", self.model)
+        names = {id(p): n for n, p in inner.named_parameters()}
+        params = self.Gparams if kind == "G" else self.Dparams
+        return {names[id(p)]: c for p, c in zip(params, g.report.tolist()) if c}
+
+    def exchange_and_step(self, optimizer, params, kind=None):
+        """optimizer step of one half-step; with more than one rank: pack -> all-reduce (SUM) -> Adam reading the bucket.
+        With ``opt.skip_nonfinite_steps`` the gradients Adam reads (the reduced bucket with more than one rank: the same bytes
+        on every rank) are scanned first and a non-finite one drops the update of the half-step ``kind``."""
+        guard = self.nonfinite_guard(kind) if kind is not None and self.nonfinite_guard_on() else None
+        kw = {} if guard is None else {"guard": guard}
         if self.world > 1:
-            optimizer.step(grads=self.model.reduce_to_bucket(params), grad_scale=1.0 / self.world)
+            optimizer.step(grads=self.model.reduce_to_bucket(params), grad_scale=1.0 / self.world, **kw)
         else:
-            optimizer.step()
+            optimizer.step(**kw)
 
     @staticmethod
     def set_requires_grad(params, requires_grad):
@@ -170,7 +242,7 @@ class SwappingAutoencoderOptimizer:
         g_losses, g_metrics = self.model(images, None, None, command="compute_generator_losses")
         sum(v.mean() for v in g_losses.values()).backward()
         if step:
-            self.exchange_and_step(self.optimizer_G, self.Gparams)
+            self.exchange_and_step(self.optimizer_G, self.Gparams, kind="G")
         g_losses.update(g_metrics)
         return g_losses
 
@@ -184,7 +256,7 @@ class SwappingAutoencoderOptimizer:
         d_losses["_sp"], d_losses["_gl"] = sp.detach(), gl.detach()
         d_losses.update({"_metric:" + k: v for k, v in d_metrics.items()})
         if step:
-            self.exchange_and_step(self.optimizer_D, self.Dparams)
+            self.exchange_and_step(self.optimizer_D, self.Dparams, kind="D")
         return d_losses
 
     def _r1_body(self, images, step=True):
@@ -194,7 +266,7 @@ class SwappingAutoencoderOptimizer:
         r1_losses = self.model(images, command="compute_R1_loss")
         (sum(v.mean() for v in r1_losses.values()) * self.opt.R1_once_every).backward()
         if step:
-            self.exchange_and_step(self.optimizer_D, self.Dparams)
+            self.exchange_and_step(self.optimizer_D, self.Dparams, kind="R1")
         return r1_losses
 
     def _run(self, kind, images):
@@ -232,15 +304,22 @@ class SwappingAutoencoderOptimizer:
     # ------------------------------------------------------------------ checkpointing (SURVEY.md §8 f3)
     def state_dict(self):
         """Adam state of both groups (torch.optim.Adam's format) + the schedule counters.  The reference never saves this
-        (optimizers/base_optimizer.py has no state I/O): resuming there restarts Adam's moments from zero."""
-        return {"optimizer_G": self.optimizer_G.state_dict(), "optimizer_D": self.optimizer_D.state_dict(),
-                "train_mode_counter": self.train_mode_counter, "discriminator_iter_counter": self.discriminator_iter_counter}
+        (optimizers/base_optimizer.py has no state I/O): resuming there restarts Adam's moments from zero.  With
+        ``opt.skip_nonfinite_steps`` the guard's skip counters (``nonfinite_steps()``) are saved as well."""
+        sd = {"optimizer_G": self.optimizer_G.state_dict(), "optimizer_D": self.optimizer_D.state_dict(),
+              "train_mode_counter": self.train_mode_counter, "discriminator_iter_counter": self.discriminator_iter_counter}
+        if self.nonfinite_guard_on():
+            sd["nonfinite_steps"] = self.nonfinite_steps()
+        return sd
 
     def load_state_dict(self, sd):
         self.optimizer_G.load_state_dict(sd["optimizer_G"])
         self.optimizer_D.load_state_dict(sd["optimizer_D"])
         self.train_mode_counter = int(sd.get("train_mode_counter", 0))
         self.discriminator_iter_counter = int(sd.get("discriminator_iter_counter", 0))
+        if "nonfinite_steps" in sd:
+            counts = [int(sd["nonfinite_steps"].get(k, 0)) for k in NONFINITE_KINDS]
+            self._nonfinite_counters().copy_(torch.tensor(counts, dtype=torch.int64))     # in place: captured graphs hold it
 
     def _optimizer_path(self, total_steps_so_far=None):
         inner = getattr(self.model, "singlegpu_model", self.model)

@@ -37,6 +37,10 @@ def default_options(**overrides):
         # extension: losses are read back with one asynchronous copy per half-step and the host only waits when a value is
         # looked at (util.LazyLosses); False: the reference's blocking to_numpy
         async_loss_readback=True,
+        # extension: scan the gradients of every half-step on the device and drop its Adam update when one of them holds a NaN
+        # or an Inf (parameters, moments and step counts stay bitwise unchanged); nonfinite_steps() / nonfinite_report() tell
+        # how often and where (optimizer.NonfiniteGuard)
+        skip_nonfinite_steps=False,
     )
     for k, v in overrides.items():
         setattr(opt, k, v)
