@@ -29,7 +29,7 @@ def audit(name, fn):
 
 
 for mod in (conv, upfirdn2d):
-    mod._nhwc = audit(mod.__name__.split(".")[-1] + "._nhwc", mod._nhwc)
+    mod.nhwc = audit(mod.__name__.split(".")[-1] + ".nhwc", mod.nhwc)
 fused_act._cl = audit("fused_act._cl", fused_act._cl)
 
 opt = S.default_options(num_gpus=1, batch_size=int(os.environ.get("B", "8")))

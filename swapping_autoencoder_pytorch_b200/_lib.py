@@ -13,6 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libsae_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
 
 SAE_ABI_VERSION = 16
+SAE_E_UNSUPPORTED = -3        # a valid request no kernel of this build takes (header: SAE_E_*)
 
 c_float_p = ctypes.c_void_p   # raw device pointers travel as integers
 c_stream = ctypes.c_void_p

@@ -48,8 +48,23 @@ def parse_deterministic(value):
     return v == "1"
 
 
+def nhwc(t):
+    """logical NCHW tensor -> the physical NHWC storage the kernels take (contiguous [N, H, W, C])"""
+    return t.permute(0, 2, 3, 1).contiguous()
+
+
+def nchw(t):
+    """physical NHWC tensor -> its logical NCHW view (no copy)"""
+    return t.permute(0, 3, 1, 2)
+
+
 def _ptr(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _floats(v):
+    """host float array (FIR tap lists)"""
+    return (ctypes.c_float * len(v))(*v)
 
 
 def _stream():
@@ -164,18 +179,37 @@ class CudaKernels:
         """the effective mode: this object's flag or torch.use_deterministic_algorithms"""
         return bool(self.deterministic) or torch.are_deterministic_algorithms_enabled()
 
-    def _call(self, name, *args):
-        """``name(*args, stream)``, or in deterministic mode its _det twin: a size query, then the call with a workspace from
-        the caching allocator (stream-ordered: the memory is reused only by work queued after this call)"""
-        if not self.deterministic_mode():
-            return getattr(self.lib, name)(*args, _stream())
-        fn = getattr(self.lib, name + "_det")
-        size = ctypes.c_int64(0)
-        rc = fn(*args, None, ctypes.byref(size), None)
-        if rc != 0:
-            return rc
-        ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=torch.device("cuda", torch.cuda.current_device()))
-        return fn(*args, _ptr(ws), ctypes.byref(size), _stream())
+    def _launch(self, device, name, *args, refusable=False):
+        """``name(*args, stream)`` on ``device`` and its current stream, raising SaeError on a failure code.  In deterministic
+        mode an entry point with a _det twin runs the twin instead: a size query, then the call with a workspace from the
+        caching allocator (stream-ordered: the memory is reused only by work queued after this call).  refusable: the
+        wrapper handles SAE_E_UNSUPPORTED (a shape the kernel does not take), which is returned instead of raised."""
+        with torch.cuda.device(device):
+            if self.deterministic_mode() and name + "_det" in _lib.DET_ENTRY_POINTS:
+                fn = getattr(self.lib, name + "_det")
+                size = ctypes.c_int64(0)
+                rc = fn(*args, None, ctypes.byref(size), None)
+                if rc == 0:
+                    ws = torch.empty(max(size.value, 1), dtype=torch.uint8, device=device)
+                    rc = fn(*args, _ptr(ws), ctypes.byref(size), _stream())
+            else:
+                rc = getattr(self.lib, name)(*args, _stream())
+        if not (refusable and rc == _lib.SAE_E_UNSUPPORTED):
+            check(rc, name)
+        return rc
+
+    def _conv(self, device, name, *args, filt=None):
+        """``_launch`` of a convolution entry point; ``args[filt]``: its filter, a tensor.  In fp32 mode the split-TF32 twin
+        (``name + "_3xtf32"``) runs instead, and the filter travels as the pair (hi, lo) = split_tf32(filter)."""
+        args = list(args)
+        if self._precision == "fp32":
+            name += "_3xtf32"
+            if filt is not None:
+                hi, lo = self.split_tf32(args[filt])
+                args[filt:filt + 1] = _ptr(hi), _ptr(lo)
+        elif filt is not None:
+            args[filt] = _ptr(args[filt])
+        self._launch(device, name, *args)
 
     def _round(self, flag=None):
         """the round_tf32 argument of a kernel call: the policy flag (or an explicit per-call value), always 0 in fp32 mode"""
@@ -187,35 +221,27 @@ class CudaKernels:
         """(hi, lo) = (rna_tf32(w), rna_tf32(w - hi)): the filter pair of the split-TF32 conv entry points"""
         w = w.contiguous()
         hi, lo = torch.empty_like(w), torch.empty_like(w)
-        with torch.cuda.device(w.device):
-            check(self.lib.sae_split_tf32(_ptr(w), _ptr(hi), _ptr(lo), w.numel(), _stream()), "sae_split_tf32")
+        self._launch(w.device, "sae_split_tf32", _ptr(w), _ptr(hi), _ptr(lo), w.numel())
         return hi, lo
 
     # ------------------------------------------------------------------ FIR
     def upfirdn2d(self, x, kernel, up_x, up_y, down_x, down_y, pad_x0, pad_x1, pad_y0, pad_y1, taps=None):
         """taps: optional host-side 1-D factors (taps_y, taps_x) with kernel == outer(taps_y, taps_x); supplied by
-        the Blur modules, which build their kernels from 1-D tap lists — selects the separable fast path."""
+        the Blur modules, which build their kernels from 1-D tap lists — selects the separable fast path wherever that
+        kernel takes the shape."""
         _need_cuda(x, kernel)
         n, h, w, c = x.shape
         kh, kw = kernel.shape
         oh = (h * up_y + pad_y0 + pad_y1 - kh) // down_y + 1
         ow = (w * up_x + pad_x0 + pad_x1 - kw) // down_x + 1
         out = torch.empty((n, oh, ow, c), device=x.device, dtype=x.dtype)
-        ud = (up_x, down_x)
-        if up_x == up_y and down_x == down_y and ud in ((1, 1), (1, 2), (2, 1)) and c % 4 == 0 \
-                and n * oh * ow * (c // 4) < 2 ** 32 and x.data_ptr() % 16 == 0 and n > 0:
-            if taps is not None and len(taps[0]) == kh and len(taps[1]) == kw and kh == kw and kh <= 4:
-                ty = (ctypes.c_float * kh)(*taps[0])
-                tx = (ctypes.c_float * kw)(*taps[1])
-                with torch.cuda.device(x.device):
-                    check(self.lib.sae_upfirdn2d_separable(_ptr(x), ty, tx, _ptr(out), n, h, w, c, kh, kw, up_x, down_x, pad_x0,
-                                                           pad_x1, pad_y0, pad_y1, self._round(), _stream()),
-                          "sae_upfirdn2d_separable")
+        pads = (pad_x0, pad_x1, pad_y0, pad_y1)
+        if taps is not None and up_x == up_y and down_x == down_y and (len(taps[0]), len(taps[1])) == (kh, kw):
+            if self._launch(x.device, "sae_upfirdn2d_separable", _ptr(x), _floats(taps[0]), _floats(taps[1]), _ptr(out), n, h, w,
+                            c, kh, kw, up_x, down_x, *pads, self._round(), refusable=True) != _lib.SAE_E_UNSUPPORTED:
                 return out
-        with torch.cuda.device(x.device):
-            check(self.lib.sae_upfirdn2d(_ptr(x), _ptr(kernel), _ptr(out), n, h, w, c, kh, kw, up_x, up_y,
-                                         down_x, down_y, pad_x0, pad_x1, pad_y0, pad_y1, self._round(), _stream()),
-                  "sae_upfirdn2d")
+        self._launch(x.device, "sae_upfirdn2d", _ptr(x), _ptr(kernel), _ptr(out), n, h, w, c, kh, kw, up_x, up_y, down_x, down_y,
+                     *pads, self._round())
         return out
 
     # ------------------------------------------------------------- bias/act
@@ -224,11 +250,9 @@ class CudaKernels:
         _need_cuda(x, bias, ref, noise, noise_weight)
         out = torch.empty_like(x)
         c = x.shape[-1]
-        with torch.cuda.device(x.device):
-            check(self.lib.sae_fused_bias_act(_ptr(x), _ptr(bias), _ptr(ref), _ptr(out), x.numel(), 1,
-                                              bias.numel() if bias is not None else 1, act, grad, alpha, scale,
-                                              _ptr(noise), _ptr(noise_weight), c, self._round(), _stream()),
-                  "sae_fused_bias_act")
+        self._launch(x.device, "sae_fused_bias_act", _ptr(x), _ptr(bias), _ptr(ref), _ptr(out), x.numel(), 1,
+                     bias.numel() if bias is not None else 1, act, grad, alpha, scale, _ptr(noise), _ptr(noise_weight), c,
+                     self._round())
         return out
 
     def bias_act_backward(self, grad_out, out, alpha, scale, want_bias=True, noise=None, mask=None):
@@ -238,9 +262,8 @@ class CudaKernels:
         gi = torch.empty_like(out)
         gb = torch.zeros(c, device=out.device, dtype=out.dtype) if want_bias else None
         gnw = torch.zeros(1, device=out.device, dtype=out.dtype) if noise is not None else None
-        with torch.cuda.device(out.device):
-            check(self._call("sae_bias_act_backward", _ptr(grad_out), _ptr(out), _ptr(gi), _ptr(gb), out.numel(), c,
-                             alpha, scale, _ptr(noise), c, _ptr(gnw), self._round(), _ptr(mask)), "sae_bias_act_backward")
+        self._launch(out.device, "sae_bias_act_backward", _ptr(grad_out), _ptr(out), _ptr(gi), _ptr(gb), out.numel(), c, alpha,
+                     scale, _ptr(noise), c, _ptr(gnw), self._round(), _ptr(mask))
         return gi, gb, gnw
 
     def fir_act_backward(self, grad, taps, act_out, pad, alpha, scale, want_bias=True, mask=None):
@@ -252,19 +275,16 @@ class CudaKernels:
         kh, kw = len(taps[0]), len(taps[1])
         px0, px1, py0, py1 = pad
         oh, ow = h + py0 + py1 - kh + 1, w + px0 + px1 - kw + 1
-        if (c % 32 != 0 or kh != kw or kh not in (3, 4) or oh < 8 or ow < 8 or n == 0 or grad.data_ptr() % 16 != 0
-                or tuple(act_out.shape) != (n, oh, ow, c) or not self.fused_fir_act):
+        # the deterministic twin also takes outputs under 8 x 8, which the fused kernel refuses: those stay on the two-launch
+        # path in both modes
+        if tuple(act_out.shape) != (n, oh, ow, c) or oh < 8 or ow < 8 or not self.fused_fir_act:
             return None
         gi = torch.empty_like(act_out)
         gb = torch.zeros(c, device=grad.device, dtype=grad.dtype) if want_bias else None
-        ty = (ctypes.c_float * kh)(*taps[0])
-        tx = (ctypes.c_float * kw)(*taps[1])
-        with torch.cuda.device(grad.device):
-            rc = self._call("sae_fir_act_backward", _ptr(grad), ty, tx, _ptr(act_out), _ptr(gi), _ptr(gb), n, h, w, c, kh, kw,
-                            px0, px1, py0, py1, alpha, scale, self._round(), _ptr(mask))
-        if rc == -3:            # SAE_E_UNSUPPORTED: e.g. no TMA on this device
+        if self._launch(grad.device, "sae_fir_act_backward", _ptr(grad), _floats(taps[0]), _floats(taps[1]), _ptr(act_out),
+                        _ptr(gi), _ptr(gb), n, h, w, c, kh, kw, px0, px1, py0, py1, alpha, scale, self._round(), _ptr(mask),
+                        refusable=True) == _lib.SAE_E_UNSUPPORTED:
             return None
-        check(rc, "sae_fir_act_backward")
         return gi, gb
 
     def fir_bias_act(self, x, taps, pad, bias, noise, noise_weight, alpha, scale):
@@ -275,19 +295,12 @@ class CudaKernels:
         n, h, w, c = x.shape
         kh, kw = len(taps[0]), len(taps[1])
         px0, px1, py0, py1 = pad
-        oh, ow = h + py0 + py1 - kh + 1, w + px0 + px1 - kw + 1
-        if c % 32 != 0 or kh != kw or kh not in (3, 4) or oh < 8 or ow < 8 or n == 0 or x.data_ptr() % 16 != 0:
-            return None
-        out = torch.empty((n, oh, ow, c), device=x.device, dtype=x.dtype)
+        out = torch.empty((n, h + py0 + py1 - kh + 1, w + px0 + px1 - kw + 1, c), device=x.device, dtype=x.dtype)
         mask = self._new_act_mask(out, 3, True)
-        ty = (ctypes.c_float * kh)(*taps[0])
-        tx = (ctypes.c_float * kw)(*taps[1])
-        with torch.cuda.device(x.device):
-            rc = self.lib.sae_fir_bias_act(_ptr(x), ty, tx, _ptr(bias), _ptr(noise), _ptr(noise_weight), _ptr(out), n, h, w, c,
-                                           kh, kw, px0, px1, py0, py1, alpha, scale, self._round(), _ptr(mask), _stream())
-        if rc == -3:
+        if self._launch(x.device, "sae_fir_bias_act", _ptr(x), _floats(taps[0]), _floats(taps[1]), _ptr(bias), _ptr(noise),
+                        _ptr(noise_weight), _ptr(out), n, h, w, c, kh, kw, px0, px1, py0, py1, alpha, scale, self._round(),
+                        _ptr(mask), refusable=True) == _lib.SAE_E_UNSUPPORTED:
             return None
-        check(rc, "sae_fir_bias_act")
         if mask is not None:
             out._sae_act_mask = mask
         return out
@@ -297,9 +310,7 @@ class CudaKernels:
         _need_cuda(x, s)
         n, h, w, c = x.shape
         out = torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            check(self.lib.sae_modulate(_ptr(x), _ptr(s), _ptr(out), n, h * w, c, self._round(), _stream()),
-                  "sae_modulate")
+        self._launch(x.device, "sae_modulate", _ptr(x), _ptr(s), _ptr(out), n, h * w, c, self._round())
         return out
 
     def modulate_backward(self, dy, x, s):
@@ -307,9 +318,7 @@ class CudaKernels:
         n, h, w, c = x.shape
         dx = torch.empty_like(x)
         ds = torch.zeros_like(s)
-        with torch.cuda.device(x.device):
-            check(self._call("sae_modulate_backward", _ptr(dy), _ptr(x), _ptr(s), _ptr(dx), _ptr(ds), n, h * w, c,
-                             self._round()), "sae_modulate_backward")
+        self._launch(x.device, "sae_modulate_backward", _ptr(dy), _ptr(x), _ptr(s), _ptr(dx), _ptr(ds), n, h * w, c, self._round())
         return dx, ds
 
     # ------------------------------------------------------- residual merge
@@ -317,9 +326,7 @@ class CudaKernels:
         """(a + b) * scale, or a * scale when b is None; any shape, a and b contiguous with identical layout"""
         _need_cuda(a, b)
         out = torch.empty_like(a)
-        with torch.cuda.device(a.device):
-            check(self.lib.sae_add_scale(_ptr(a), _ptr(b), _ptr(out), a.numel(), scale, self._round(), _stream()),
-                  "sae_add_scale")
+        self._launch(a.device, "sae_add_scale", _ptr(a), _ptr(b), _ptr(out), a.numel(), scale, self._round())
         return out
 
     def upsample2x_add_scale(self, skip, res, scale):
@@ -328,9 +335,7 @@ class CudaKernels:
         n, h, w, c = skip.shape
         assert tuple(res.shape) == (n, 2 * h, 2 * w, c)
         out = torch.empty_like(res)
-        with torch.cuda.device(res.device):
-            check(self.lib.sae_upsample2x_add_scale(_ptr(skip), _ptr(res), _ptr(out), n, h, w, c, scale,
-                                                    self._round(), _stream()), "sae_upsample2x_add_scale")
+        self._launch(res.device, "sae_upsample2x_add_scale", _ptr(skip), _ptr(res), _ptr(out), n, h, w, c, scale, self._round())
         return out
 
     def upsample2x_backward(self, dy, scale):
@@ -338,9 +343,7 @@ class CudaKernels:
         _need_cuda(dy)
         n, oh, ow, c = dy.shape
         out = torch.empty((n, oh // 2, ow // 2, c), device=dy.device, dtype=dy.dtype)
-        with torch.cuda.device(dy.device):
-            check(self.lib.sae_upsample2x_backward(_ptr(dy), _ptr(out), n, oh // 2, ow // 2, c, scale,
-                                                   self._round(), _stream()), "sae_upsample2x_backward")
+        self._launch(dy.device, "sae_upsample2x_backward", _ptr(dy), _ptr(out), n, oh // 2, ow // 2, c, scale, self._round())
         return out
 
     def pad_channels(self, x, c_out):
@@ -351,9 +354,8 @@ class CudaKernels:
         if h > 1 and x.stride(2) != w * x.stride(3):
             x = x.contiguous()
         out = torch.empty((n, h, w, c_out), device=x.device, dtype=x.dtype)
-        with torch.cuda.device(x.device):
-            check(self.lib.sae_pad_channels(_ptr(x), _ptr(out), n, h * w, c, c_out, x.stride(0), x.stride(1), x.stride(3),
-                                            self._round(), _stream()), "sae_pad_channels")
+        self._launch(x.device, "sae_pad_channels", _ptr(x), _ptr(out), n, h * w, c, c_out, x.stride(0), x.stride(1), x.stride(3),
+                     self._round())
         return out
 
     def reflect_pad(self, x, pads):
@@ -362,8 +364,7 @@ class CudaKernels:
         n, h, w, c = x.shape
         pl, pr, pt, pb = pads
         out = torch.empty((n, h + pt + pb, w + pl + pr, c), device=x.device, dtype=x.dtype)
-        with torch.cuda.device(x.device):
-            check(self.lib.sae_reflect_pad(_ptr(x), _ptr(out), n, h, w, c, pl, pr, pt, pb, _stream()), "sae_reflect_pad")
+        self._launch(x.device, "sae_reflect_pad", _ptr(x), _ptr(out), n, h, w, c, pl, pr, pt, pb)
         return out
 
     def reflect_pad_backward(self, dy, pads):
@@ -371,9 +372,7 @@ class CudaKernels:
         n, oh, ow, c = dy.shape
         pl, pr, pt, pb = pads
         dx = torch.empty((n, oh - pt - pb, ow - pl - pr, c), device=dy.device, dtype=dy.dtype)
-        with torch.cuda.device(dy.device):
-            check(self.lib.sae_reflect_pad_backward(_ptr(dy), _ptr(dx), n, oh - pt - pb, ow - pl - pr, c, pl, pr, pt, pb,
-                                                    _stream()), "sae_reflect_pad_backward")
+        self._launch(dy.device, "sae_reflect_pad_backward", _ptr(dy), _ptr(dx), n, oh - pt - pb, ow - pl - pr, c, pl, pr, pt, pb)
         return dx
 
     def filter_prep(self, w_oihw, scale, want_crsk=True):
@@ -382,9 +381,7 @@ class CudaKernels:
         k, c, r, s = w_oihw.shape
         krsc = torch.empty((k, r, s, c), device=w_oihw.device, dtype=w_oihw.dtype)
         crsk = torch.empty((c, r, s, k), device=w_oihw.device, dtype=w_oihw.dtype) if want_crsk else None
-        with torch.cuda.device(w_oihw.device):
-            check(self.lib.sae_filter_prep(_ptr(w_oihw), _ptr(krsc), _ptr(crsk), k, c, r, s, scale, self._round(),
-                                           _stream()), "sae_filter_prep")
+        self._launch(w_oihw.device, "sae_filter_prep", _ptr(w_oihw), _ptr(krsc), _ptr(crsk), k, c, r, s, scale, self._round())
         return krsc, crsk
 
     def filter_unprep(self, d_krsc, scale):
@@ -392,8 +389,7 @@ class CudaKernels:
         _need_cuda(d_krsc)
         k, r, s, c = d_krsc.shape
         out = torch.empty((k, c, r, s), device=d_krsc.device, dtype=d_krsc.dtype)
-        with torch.cuda.device(d_krsc.device):
-            check(self.lib.sae_filter_unprep(_ptr(d_krsc), _ptr(out), k, c, r, s, scale, _stream()), "sae_filter_unprep")
+        self._launch(d_krsc.device, "sae_filter_unprep", _ptr(d_krsc), _ptr(out), k, c, r, s, scale)
         return out
 
     def _filter(self, w):
@@ -402,8 +398,7 @@ class CudaKernels:
         if not self._round():
             return w
         out = torch.empty_like(w)
-        with torch.cuda.device(w.device):
-            check(self.lib.sae_round_tf32(_ptr(w), _ptr(out), w.numel(), _stream()), "sae_round_tf32")
+        self._launch(w.device, "sae_round_tf32", _ptr(w), _ptr(out), w.numel())
         return out
 
     # ----------------------------------------------------------------- conv
@@ -440,14 +435,7 @@ class CudaKernels:
         if epi.get("act", 1) == 3 and self.act_masks:
             mask = self._new_act_mask(y, 3, impl == 2 or (impl == 0 and self.conv_impl_for(g, 0) == 2))
         e = self._epi(act_mask=mask, **epi)
-        with torch.cuda.device(x.device):
-            if self._precision == "fp32":
-                hi, lo = self.split_tf32(w_krsc)
-                check(self._call("sae_conv2d_fprop_3xtf32", _ptr(x), _ptr(hi), _ptr(lo), _ptr(y), ctypes.byref(g), ctypes.byref(e),
-                                 impl), "sae_conv2d_fprop_3xtf32")
-            else:
-                check(self._call("sae_conv2d_fprop", _ptr(x), _ptr(w_krsc), _ptr(y), ctypes.byref(g), ctypes.byref(e), impl),
-                      "sae_conv2d_fprop")
+        self._conv(x.device, "sae_conv2d_fprop", _ptr(x), w_krsc, _ptr(y), ctypes.byref(g), ctypes.byref(e), impl, filt=1)
         if mask is not None:
             y._sae_act_mask = mask
         return y
@@ -462,14 +450,7 @@ class CudaKernels:
         dx = torch.empty((g.N, g.H, g.W, g.C), device=dy.device, dtype=dy.dtype)
         e = self._epi(**epi)
         impl = self.conv_impl if impl is None else impl
-        with torch.cuda.device(dy.device):
-            if self._precision == "fp32":
-                hi, lo = self.split_tf32(wt)
-                check(self._call("sae_conv2d_dgrad_3xtf32", _ptr(dy), _ptr(hi), _ptr(lo), _ptr(dx), ctypes.byref(g), ctypes.byref(e),
-                                 impl), "sae_conv2d_dgrad_3xtf32")
-            else:
-                check(self._call("sae_conv2d_dgrad", _ptr(dy), _ptr(wt), _ptr(dx), ctypes.byref(g), ctypes.byref(e), impl),
-                      "sae_conv2d_dgrad")
+        self._conv(dy.device, "sae_conv2d_dgrad", _ptr(dy), wt, _ptr(dx), ctypes.byref(g), ctypes.byref(e), impl, filt=1)
         return dx
 
     def conv_wgrad(self, dy, x, g, impl=None):
@@ -478,9 +459,8 @@ class CudaKernels:
         assert tuple(dy.shape) == (g.N, g.P, g.Q, g.K) and tuple(x.shape) == (g.N, g.H, g.W, g.C), \
             (tuple(dy.shape), tuple(x.shape), g.key())
         dw = torch.zeros((g.K, g.R, g.S, g.C), device=dy.device, dtype=dy.dtype)
-        name = "sae_conv2d_wgrad_3xtf32" if self._precision == "fp32" else "sae_conv2d_wgrad"
-        with torch.cuda.device(dy.device):
-            check(self._call(name, _ptr(dy), _ptr(x), _ptr(dw), ctypes.byref(g), self.conv_impl if impl is None else impl), name)
+        self._conv(dy.device, "sae_conv2d_wgrad", _ptr(dy), _ptr(x), _ptr(dw), ctypes.byref(g),
+                   self.conv_impl if impl is None else impl)
         return dw
 
     # ------------------------------------------------ style-modulated conv, per-sample filters
@@ -495,9 +475,7 @@ class CudaKernels:
         n = s.shape[0]
         a = torch.empty((n, k, r, s_, c), device=s.device, dtype=s.dtype) if want_krsc else None
         b = torch.empty((n, c, r, s_, k), device=s.device, dtype=s.dtype) if want_crsk else None
-        with torch.cuda.device(s.device):
-            check(self.lib.sae_filter_modulate(_ptr(w_krsc), _ptr(s), _ptr(a), _ptr(b), n, k, c, r, s_, self._round(),
-                                               _stream()), "sae_filter_modulate")
+        self._launch(s.device, "sae_filter_modulate", _ptr(w_krsc), _ptr(s), _ptr(a), _ptr(b), n, k, c, r, s_, self._round())
         return a, b
 
     def conv_fprop_per_sample(self, x, w_nkrsc, g, **epi):
@@ -506,14 +484,7 @@ class CudaKernels:
         y = torch.empty((g.N, g.P, g.Q, g.K), device=x.device, dtype=x.dtype)
         mask = self._new_act_mask(y, epi.get("act", 1), True)          # only the wgmma kernel implements per-sample filters
         e = self._epi(act_mask=mask, **epi)
-        with torch.cuda.device(x.device):
-            if self._precision == "fp32":
-                hi, lo = self.split_tf32(w_nkrsc)
-                check(self.lib.sae_conv2d_fprop_per_sample_3xtf32(_ptr(x), _ptr(hi), _ptr(lo), _ptr(y), ctypes.byref(g),
-                                                                  ctypes.byref(e), _stream()), "sae_conv2d_fprop_per_sample_3xtf32")
-            else:
-                check(self.lib.sae_conv2d_fprop_per_sample(_ptr(x), _ptr(w_nkrsc), _ptr(y), ctypes.byref(g), ctypes.byref(e),
-                                                           _stream()), "sae_conv2d_fprop_per_sample")
+        self._conv(x.device, "sae_conv2d_fprop_per_sample", _ptr(x), w_nkrsc, _ptr(y), ctypes.byref(g), ctypes.byref(e), filt=1)
         if mask is not None:
             y._sae_act_mask = mask
         return y
@@ -523,14 +494,7 @@ class CudaKernels:
         _need_cuda(dy, w_ncrsk)
         dx = torch.empty((g.N, g.H, g.W, g.C), device=dy.device, dtype=dy.dtype)
         e = self._epi(**epi)
-        with torch.cuda.device(dy.device):
-            if self._precision == "fp32":
-                hi, lo = self.split_tf32(w_ncrsk)
-                check(self.lib.sae_conv2d_dgrad_per_sample_3xtf32(_ptr(dy), _ptr(hi), _ptr(lo), _ptr(dx), ctypes.byref(g),
-                                                                  ctypes.byref(e), _stream()), "sae_conv2d_dgrad_per_sample_3xtf32")
-            else:
-                check(self.lib.sae_conv2d_dgrad_per_sample(_ptr(dy), _ptr(w_ncrsk), _ptr(dx), ctypes.byref(g), ctypes.byref(e),
-                                                           _stream()), "sae_conv2d_dgrad_per_sample")
+        self._conv(dy.device, "sae_conv2d_dgrad_per_sample", _ptr(dy), w_ncrsk, _ptr(dx), ctypes.byref(g), ctypes.byref(e), filt=1)
         return dx
 
     def conv_wgrad_modulated(self, dy, x, s, w_krsc, g):
@@ -538,9 +502,8 @@ class CudaKernels:
         _need_cuda(dy, x, s, w_krsc)
         dw = torch.zeros((g.K, g.R, g.S, g.C), device=dy.device, dtype=dy.dtype)
         ds = torch.zeros((g.N, g.C), device=dy.device, dtype=dy.dtype)
-        name = "sae_conv2d_wgrad_modulated_3xtf32" if self._precision == "fp32" else "sae_conv2d_wgrad_modulated"
-        with torch.cuda.device(dy.device):
-            check(self._call(name, _ptr(dy), _ptr(x), _ptr(s), _ptr(w_krsc), _ptr(dw), _ptr(ds), ctypes.byref(g)), name)
+        self._conv(dy.device, "sae_conv2d_wgrad_modulated", _ptr(dy), _ptr(x), _ptr(s), _ptr(w_krsc), _ptr(dw), _ptr(ds),
+                   ctypes.byref(g))
         return dw, ds
 
     def conv_impl_for(self, g, direction):
@@ -548,14 +511,11 @@ class CudaKernels:
 
     # --------------------------------------------------------------- bucket
     def bucket_pack(self, ptrs, offsets, sizes, n, bucket):
-        with torch.cuda.device(bucket.device):
-            check(self.lib.sae_bucket_pack(_ptr(ptrs), _ptr(offsets), _ptr(sizes), n, _ptr(bucket), bucket.numel(),
-                                           _stream()), "sae_bucket_pack")
+        self._launch(bucket.device, "sae_bucket_pack", _ptr(ptrs), _ptr(offsets), _ptr(sizes), n, _ptr(bucket), bucket.numel())
 
     def bucket_unpack(self, ptrs, offsets, sizes, n, bucket, scale):
-        with torch.cuda.device(bucket.device):
-            check(self.lib.sae_bucket_unpack(_ptr(ptrs), _ptr(offsets), _ptr(sizes), n, _ptr(bucket), bucket.numel(),
-                                             scale, _stream()), "sae_bucket_unpack")
+        self._launch(bucket.device, "sae_bucket_unpack", _ptr(ptrs), _ptr(offsets), _ptr(sizes), n, _ptr(bucket), bucket.numel(),
+                     scale)
 
 
     # ----------------------------------------------------------------- Adam
@@ -567,7 +527,6 @@ class CudaKernels:
         the flat ``exp_avg`` / ``exp_avg_sq``; steps: device float tensor, one count per parameter.  cache: the caller's
         ``PointerTables`` (device copies of the address lists).  skip: optional one-element device int64 tensor (the total of
         ``nonfinite_count``); the kernels drop the whole update when it is non-zero (sae_adam_step_guarded)."""
-        dev = exp_avg.device
         p_tab = cache.get(tuple(p.data_ptr() for p in params))
         g_tab = cache.get(tuple(0 if g is None else g.data_ptr() for g in grads))
         for g in grads:
@@ -575,12 +534,11 @@ class CudaKernels:
                 raise _lib.SaeError("adam_step: gradients must be contiguous fp32 CUDA tensors")
         args = (_ptr(p_tab), _ptr(g_tab), _ptr(offsets), _ptr(sizes), len(params), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(steps), lr,
                 beta1, beta2, eps, grad_scale)
-        with torch.cuda.device(dev):
-            if skip is None:
-                check(self.lib.sae_adam_step(*args, _stream()), "sae_adam_step")
-            else:
-                _need_int64(skip)
-                check(self.lib.sae_adam_step_guarded(*args, _ptr(skip), _stream()), "sae_adam_step_guarded")
+        if skip is None:
+            self._launch(exp_avg.device, "sae_adam_step", *args)
+        else:
+            _need_int64(skip)
+            self._launch(exp_avg.device, "sae_adam_step_guarded", *args, _ptr(skip))
 
     def nonfinite_count(self, tensors, sizes, counts, cache):
         """counts[i] += number of NaN / +-Inf elements of tensors[i] (None: skipped), counts[n] += their sum; one launch.
@@ -592,9 +550,7 @@ class CudaKernels:
         if counts.numel() != len(tensors) + 1 or sizes.numel() != len(tensors):
             raise _lib.SaeError("nonfinite_count: counts needs n + 1 entries and sizes n")
         tab = cache.get(tuple(0 if t is None else t.data_ptr() for t in tensors))
-        with torch.cuda.device(counts.device):
-            check(self.lib.sae_nonfinite_count(_ptr(tab), _ptr(sizes), len(tensors), _ptr(counts), _stream()),
-                  "sae_nonfinite_count")
+        self._launch(counts.device, "sae_nonfinite_count", _ptr(tab), _ptr(sizes), len(tensors), _ptr(counts))
 
     # ----------------------------------------------------------------- ToRGB
     def torgb_forward(self, x, s, w, bias, wscale):
@@ -602,9 +558,8 @@ class CudaKernels:
         _need_cuda(x, s, w, bias)
         n, h, wd, c = x.shape
         y = torch.empty((n, h, wd, 4), device=x.device, dtype=x.dtype)
-        with torch.cuda.device(x.device):
-            check(self.lib.sae_torgb_forward(_ptr(x), _ptr(s), _ptr(w), _ptr(bias), _ptr(y), n, h, wd, c, wscale,
-                                             self._round(), _stream()), "sae_torgb_forward")
+        self._launch(x.device, "sae_torgb_forward", _ptr(x), _ptr(s), _ptr(w), _ptr(bias), _ptr(y), n, h, wd, c, wscale,
+                     self._round())
         return y
 
     def torgb_backward(self, dy, x, s, w, wscale, want_dx=True, want_gw=True):
@@ -614,9 +569,8 @@ class CudaKernels:
         n, h, wd, c = x.shape
         dx = torch.empty_like(x) if want_dx else None
         gw = torch.zeros((n, 3, c), device=x.device, dtype=x.dtype) if want_gw else None
-        with torch.cuda.device(x.device):
-            check(self._call("sae_torgb_backward", _ptr(dy), _ptr(x), _ptr(s), _ptr(w), _ptr(dx), _ptr(gw), n, h, wd, c, wscale,
-                             dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3), self._round()), "sae_torgb_backward")
+        self._launch(x.device, "sae_torgb_backward", _ptr(dy), _ptr(x), _ptr(s), _ptr(w), _ptr(dx), _ptr(gw), n, h, wd, c, wscale,
+                     dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3), self._round())
         return dx, gw
 
     # ----------------------------------------------------------------- crops
@@ -629,10 +583,8 @@ class CudaKernels:
         if out is None:
             out = torch.empty((q, size, size, c_pad), device=x.device, dtype=x.dtype)
         assert tuple(out.shape) == (q, size, size, c_pad) and out.is_contiguous()
-        with torch.cuda.device(x.device):
-            check(self.lib.sae_crop_gather(_ptr(x), _ptr(flip), _ptr(scale), _ptr(offset), _ptr(out), q, num_crops, c, h, w, size,
-                                           c_pad, x.stride(0), x.stride(1), x.stride(2), x.stride(3), self._round(),
-                                           _stream()), "sae_crop_gather")
+        self._launch(x.device, "sae_crop_gather", _ptr(x), _ptr(flip), _ptr(scale), _ptr(offset), _ptr(out), q, num_crops, c, h, w,
+                     size, c_pad, x.stride(0), x.stride(1), x.stride(2), x.stride(3), self._round())
         return out
 
     def crop_gather_backward(self, dy, flip, scale, offset, num_crops, c, h, w):
@@ -640,11 +592,10 @@ class CudaKernels:
         _need_cuda(dy, flip, scale, offset, strided=True)
         q, s = dy.shape[0], dy.shape[2]
         dx = torch.empty((q // num_crops, c, h, w), device=dy.device, dtype=dy.dtype)
-        with torch.cuda.device(dy.device):
-            check(self.lib.sae_crop_gather_backward(_ptr(dy), _ptr(flip), _ptr(scale), _ptr(offset), _ptr(dx), q, num_crops, c, h, w,
-                                                    s, dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3), _stream()),
-                  "sae_crop_gather_backward")
+        self._launch(dy.device, "sae_crop_gather_backward", _ptr(dy), _ptr(flip), _ptr(scale), _ptr(offset), _ptr(dx), q, num_crops,
+                     c, h, w, s, dy.stride(0), dy.stride(1), dy.stride(2), dy.stride(3))
         return dx
+
 
 
 _kernels = None

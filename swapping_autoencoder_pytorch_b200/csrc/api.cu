@@ -155,62 +155,59 @@ extern "C" int sae_conv2d_query_modulated(const sae_conv_geom* g) {
     return (tc_available() && tc_per_sample_eligible(g, 0) && tc_per_sample_eligible(g, 1) && wgrad_modulated_eligible(g)) ? 1 : 0;
 }
 
-extern "C" int sae_conv2d_fprop_per_sample(const float* x, const float* w_nkrsc, float* y, const sae_conv_geom* g,
-                                           const sae_conv_epilogue* epi, void* stream) {
-    int rc = validate_geom(g, "conv2d_fprop_per_sample");
+// dir 0: forward, w [N,K,R,S,C]; dir 1: data gradient, w [N,C,R,S,K].  split: the split-TF32 twin (filter pair (w, w_lo))
+static int conv2d_per_sample(int dir, const float* x, const float* w, const float* w_lo, float* y, const sae_conv_geom* g,
+                             const sae_conv_epilogue* epi, void* stream, bool split, const char* who) {
+    int rc = validate_geom(g, who);
     if (rc) return rc;
     if (g->N == 0) return SAE_OK;
-    if (!x || !w_nkrsc || !y) return fail(SAE_E_INVALID, "conv2d_fprop_per_sample: null pointer");
-    if (!tc_available()) return fail(SAE_E_UNSUPPORTED, "conv2d_fprop_per_sample: needs the wgmma path");
-    return tc_conv_per_sample(x, w_nkrsc, y, g, 0, make_epi(epi), (cudaStream_t)stream);
+    if (!x || !w || (split && !w_lo) || !y) return fail(SAE_E_INVALID, "%s: null pointer", who);
+    if (!tc_available()) return fail(SAE_E_UNSUPPORTED, "%s: needs the wgmma path", who);
+    return tc_conv_per_sample(x, w, y, g, dir, make_epi(epi), (cudaStream_t)stream, w_lo);
+}
+
+// det: the deterministic twin (workspace protocol of det_workspace, which also refuses a null ws_bytes)
+static int conv2d_wgrad_modulated(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
+                                  const sae_conv_geom* g, void* stream, bool split, const char* who,
+                                  bool det = false, void* ws = nullptr, int64_t* ws_bytes = nullptr) {
+    int rc = validate_geom(g, who);
+    if (rc) return rc;
+    bool query;
+    if (g->N == 0) return det ? det_workspace(ws, ws_bytes, 0, who, &query) : SAE_OK;
+    if (!dy || !x || !s || !w_krsc || !dw || !ds) return fail(SAE_E_INVALID, "%s: null pointer", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (det) return conv_wgrad_modulated_det(dy, x, s, w_krsc, dw, ds, g, st, split, ws, ws_bytes, who);
+    return conv_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, st, split);
+}
+
+extern "C" int sae_conv2d_fprop_per_sample(const float* x, const float* w_nkrsc, float* y, const sae_conv_geom* g,
+                                           const sae_conv_epilogue* epi, void* stream) {
+    return conv2d_per_sample(0, x, w_nkrsc, nullptr, y, g, epi, stream, false, "conv2d_fprop_per_sample");
 }
 
 extern "C" int sae_conv2d_dgrad_per_sample(const float* dy, const float* w_ncrsk, float* dx, const sae_conv_geom* g,
                                            const sae_conv_epilogue* epi, void* stream) {
-    int rc = validate_geom(g, "conv2d_dgrad_per_sample");
-    if (rc) return rc;
-    if (g->N == 0) return SAE_OK;
-    if (!dy || !w_ncrsk || !dx) return fail(SAE_E_INVALID, "conv2d_dgrad_per_sample: null pointer");
-    if (!tc_available()) return fail(SAE_E_UNSUPPORTED, "conv2d_dgrad_per_sample: needs the wgmma path");
-    return tc_conv_per_sample(dy, w_ncrsk, dx, g, 1, make_epi(epi), (cudaStream_t)stream);
+    return conv2d_per_sample(1, dy, w_ncrsk, nullptr, dx, g, epi, stream, false, "conv2d_dgrad_per_sample");
 }
 
 extern "C" int sae_conv2d_wgrad_modulated(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
                                           const sae_conv_geom* g, void* stream) {
-    int rc = validate_geom(g, "conv2d_wgrad_modulated");
-    if (rc) return rc;
-    if (g->N == 0) return SAE_OK;
-    if (!dy || !x || !s || !w_krsc || !dw || !ds) return fail(SAE_E_INVALID, "conv2d_wgrad_modulated: null pointer");
-    return conv_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, (cudaStream_t)stream);
+    return conv2d_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, stream, false, "conv2d_wgrad_modulated");
 }
 
 extern "C" int sae_conv2d_fprop_per_sample_3xtf32(const float* x, const float* w_nkrsc_hi, const float* w_nkrsc_lo, float* y,
                                                   const sae_conv_geom* g, const sae_conv_epilogue* epi, void* stream) {
-    int rc = validate_geom(g, "conv2d_fprop_per_sample_3xtf32");
-    if (rc) return rc;
-    if (g->N == 0) return SAE_OK;
-    if (!x || !w_nkrsc_hi || !w_nkrsc_lo || !y) return fail(SAE_E_INVALID, "conv2d_fprop_per_sample_3xtf32: null pointer");
-    if (!tc_available()) return fail(SAE_E_UNSUPPORTED, "conv2d_fprop_per_sample_3xtf32: needs the wgmma path");
-    return tc_conv_per_sample(x, w_nkrsc_hi, y, g, 0, make_epi(epi), (cudaStream_t)stream, w_nkrsc_lo);
+    return conv2d_per_sample(0, x, w_nkrsc_hi, w_nkrsc_lo, y, g, epi, stream, true, "conv2d_fprop_per_sample_3xtf32");
 }
 
 extern "C" int sae_conv2d_dgrad_per_sample_3xtf32(const float* dy, const float* w_ncrsk_hi, const float* w_ncrsk_lo, float* dx,
                                                   const sae_conv_geom* g, const sae_conv_epilogue* epi, void* stream) {
-    int rc = validate_geom(g, "conv2d_dgrad_per_sample_3xtf32");
-    if (rc) return rc;
-    if (g->N == 0) return SAE_OK;
-    if (!dy || !w_ncrsk_hi || !w_ncrsk_lo || !dx) return fail(SAE_E_INVALID, "conv2d_dgrad_per_sample_3xtf32: null pointer");
-    if (!tc_available()) return fail(SAE_E_UNSUPPORTED, "conv2d_dgrad_per_sample_3xtf32: needs the wgmma path");
-    return tc_conv_per_sample(dy, w_ncrsk_hi, dx, g, 1, make_epi(epi), (cudaStream_t)stream, w_ncrsk_lo);
+    return conv2d_per_sample(1, dy, w_ncrsk_hi, w_ncrsk_lo, dx, g, epi, stream, true, "conv2d_dgrad_per_sample_3xtf32");
 }
 
 extern "C" int sae_conv2d_wgrad_modulated_3xtf32(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw,
                                                  float* ds, const sae_conv_geom* g, void* stream) {
-    int rc = validate_geom(g, "conv2d_wgrad_modulated_3xtf32");
-    if (rc) return rc;
-    if (g->N == 0) return SAE_OK;
-    if (!dy || !x || !s || !w_krsc || !dw || !ds) return fail(SAE_E_INVALID, "conv2d_wgrad_modulated_3xtf32: null pointer");
-    return conv_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, (cudaStream_t)stream, true);
+    return conv2d_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, stream, true, "conv2d_wgrad_modulated_3xtf32");
 }
 
 // ---- deterministic twins: the arguments of the entry point above, then (workspace, workspace_bytes) --------------------------
@@ -254,27 +251,16 @@ extern "C" int sae_conv2d_wgrad_3xtf32_det(const float* dy, const float* x, floa
     return conv2d_wgrad(dy, x, dw, g, impl, stream, true, "conv2d_wgrad_3xtf32_det", workspace, workspace_bytes);
 }
 
-static int wgrad_modulated_det(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw, float* ds,
-                               const sae_conv_geom* g, void* workspace, int64_t* workspace_bytes, void* stream, bool split,
-                               const char* who) {
-    int rc = validate_geom(g, who);
-    if (rc) return rc;
-    bool query;
-    if (g->N == 0) return det_workspace(workspace, workspace_bytes, 0, who, &query);
-    if (!dy || !x || !s || !w_krsc || !dw || !ds) return fail(SAE_E_INVALID, "%s: null pointer", who);
-    return conv_wgrad_modulated_det(dy, x, s, w_krsc, dw, ds, g, (cudaStream_t)stream, split, workspace, workspace_bytes, who);
-}
-
 extern "C" int sae_conv2d_wgrad_modulated_det(const float* dy, const float* x, const float* s, const float* w_krsc, float* dw,
                                               float* ds, const sae_conv_geom* g, void* workspace, int64_t* workspace_bytes,
                                               void* stream) {
-    return wgrad_modulated_det(dy, x, s, w_krsc, dw, ds, g, workspace, workspace_bytes, stream, false,
-                               "conv2d_wgrad_modulated_det");
+    return conv2d_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, stream, false, "conv2d_wgrad_modulated_det", true, workspace,
+                                  workspace_bytes);
 }
 
 extern "C" int sae_conv2d_wgrad_modulated_3xtf32_det(const float* dy, const float* x, const float* s, const float* w_krsc,
                                                      float* dw, float* ds, const sae_conv_geom* g, void* workspace,
                                                      int64_t* workspace_bytes, void* stream) {
-    return wgrad_modulated_det(dy, x, s, w_krsc, dw, ds, g, workspace, workspace_bytes, stream, true,
-                               "conv2d_wgrad_modulated_3xtf32_det");
+    return conv2d_wgrad_modulated(dy, x, s, w_krsc, dw, ds, g, stream, true, "conv2d_wgrad_modulated_3xtf32_det", true,
+                                  workspace, workspace_bytes);
 }

@@ -29,7 +29,7 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from .. import backend
-from ..backend import make_geom
+from ..backend import make_geom, nchw, nhwc
 from . import conv as C
 from .upfirdn2d import _flip_taps, upfirdn2d
 
@@ -72,14 +72,6 @@ class data_gradients_only:
     def __exit__(self, *exc):
         C.set_data_gradients_only(self.prev)
         return False
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2)
 
 
 class FirSpec:
@@ -133,7 +125,7 @@ class _FirNoiseBiasAct(Function):
     @staticmethod
     def forward(ctx, x, spec, noise, noise_weight, bias, slope, gain):
         k = backend.kernels()
-        xh = _nhwc(x)
+        xh = nhwc(x)
         p0, p1 = spec.pad
         noise_flat = noise.reshape(-1).contiguous() if noise is not None else None
         nw = noise_weight.contiguous() if noise is not None else None
@@ -145,7 +137,7 @@ class _FirNoiseBiasAct(Function):
         ctx.spec, ctx.cfg = spec, (slope, gain, tuple(noise.shape) if noise is not None else None, xh.shape[1], xh.shape[2])
         ctx.act_mask = backend.act_mask_of(out)
         ctx.save_for_backward(out, noise_flat, nw)
-        return _nchw(out)
+        return nchw(out)
 
     @staticmethod
     @once_differentiable
@@ -153,8 +145,8 @@ class _FirNoiseBiasAct(Function):
         out, noise_flat, nw = ctx.saved_tensors
         slope, gain, noise_shape, in_h, in_w = ctx.cfg
         k = backend.kernels()
-        gi, gb, gnw = k.bias_act_backward(_nhwc(dy), out, slope, gain, want_bias=True, noise=noise_flat, mask=ctx.act_mask)
-        dx = _nchw(ctx.spec.adjoint(k, gi, in_h, in_w)) if ctx.needs_input_grad[0] else None
+        gi, gb, gnw = k.bias_act_backward(nhwc(dy), out, slope, gain, want_bias=True, noise=noise_flat, mask=ctx.act_mask)
+        dx = nchw(ctx.spec.adjoint(k, gi, in_h, in_w)) if ctx.needs_input_grad[0] else None
         g_noise = None
         if noise_flat is not None and ctx.needs_input_grad[2]:
             g_noise = (gi.sum(dim=3) * nw).reshape(noise_shape)
@@ -192,7 +184,7 @@ class _ResBlockDataGrad(Function):
         k = backend.kernels()
         g1, g2, gs = geoms
         m1, m2 = masks
-        dyh = _nhwc(dy)
+        dyh = nhwc(dy)
         gi2, _, _ = k.bias_act_backward(dyh, o2, spec.slope, spec.gain2, want_bias=False, mask=m2)
         dh = k.conv_dgrad(dyh, wsk, gs, w_crsk=wst)
         dxs = spec.blur_s.adjoint(k, dh, g1.H, g1.W)
@@ -201,7 +193,7 @@ class _ResBlockDataGrad(Function):
         dx = k.conv_dgrad(gi1, w1k, g1, w_crsk=w1t, residual=dxs, res_scale=1.0)
         ctx.spec, ctx.geoms, ctx.masks = spec, geoms, masks
         ctx.save_for_backward(dyh, gi2, gi1, o1, o2, w1k, w2k, wsk)
-        return _nchw(dx)
+        return nchw(dx)
 
     @staticmethod
     @once_differentiable
@@ -212,7 +204,7 @@ class _ResBlockDataGrad(Function):
         m1, m2 = ctx.masks
         k = backend.kernels()
         need = ctx.needs_input_grad
-        vh = _nhwc(v)
+        vh = nhwc(v)
         # tangent forward through the linearised block: no biases, the saved leaky-ReLU masks
         r = None
         if need[0] or need[2]:
@@ -224,7 +216,7 @@ class _ResBlockDataGrad(Function):
         if need[0]:
             p2 = k.conv_fprop(r, w2k, g2, prepared=True)
             t2, _, _ = k.bias_act_backward(p2, o2, spec.slope, spec.gain2, want_bias=False, mask=m2)
-            d_dy = _nchw(k.conv_fprop(hv, wsk, gs, prepared=True, residual=t2, res_scale=1.0))
+            d_dy = nchw(k.conv_fprop(hv, wsk, gs, prepared=True, residual=t2, res_scale=1.0))
         unprep = k.filter_unprep
         dw1 = unprep(k.conv_wgrad(gi1, vh, g1), spec.s1) if need[1] else None
         dw2 = unprep(k.conv_wgrad(gi2, r, g2), spec.s2) if need[2] else None
@@ -241,7 +233,7 @@ class _ResBlockFused(Function):
         w1k, w1t = C.prep_filter(w1, spec.s1)
         w2k, w2t = C.prep_filter(w2, spec.s2)
         wsk, wst = C.prep_filter(ws, spec.ss)
-        xh = _nhwc(x)
+        xh = nhwc(x)
         g1 = make_geom(n, hh, ww, c, c, 3, 3, 1, 1, 1)
         o1 = k.conv_fprop(xh, w1k, g1, prepared=True, bias=b1.contiguous(), act=3, alpha=spec.slope, gain=spec.gain1)
         bl = spec.blur2.forward(k, o1)
@@ -254,7 +246,7 @@ class _ResBlockFused(Function):
         ctx.spec, ctx.geoms = spec, (g1, g2, gs)
         ctx.masks = (backend.act_mask_of(o1), backend.act_mask_of(o2))        # activation bit masks written by the two convs
         ctx.save_for_backward(x, w1, b1, w2, b2, ws, o1, bl, o2, h, w1k, w1t, w2k, w2t, wsk, wst)
-        return _nchw(y)
+        return nchw(y)
 
     @staticmethod
     def backward(ctx, dy):
@@ -277,7 +269,7 @@ class _ResBlockFused(Function):
         k = backend.kernels()
         g1, g2, gs = ctx.geoms
         m1, m2 = ctx.masks
-        dyh = _nhwc(dy)
+        dyh = nhwc(dy)
         need_x, need_w = need[0], (need[1] or need[3] or need[5])
         gi2, gb2, _ = k.bias_act_backward(dyh, o2, spec.slope, spec.gain2, want_bias=need[4], mask=m2)
         # skip branch: 1x1 conv <- decimating blur
@@ -293,10 +285,10 @@ class _ResBlockFused(Function):
             dbl = k.conv_dgrad(gi2, w2k, g2, w_crsk=w2t)
             gi1, gb1 = spec.blur2.adjoint_into_activation(k, dbl, o1, spec.slope, spec.gain1, need[2], mask=m1)
             if need[1]:
-                dw1 = k.conv_wgrad(gi1, _nhwc(x), g1)
+                dw1 = k.conv_wgrad(gi1, nhwc(x), g1)
             if need_x:
                 # the other branch's gradient is added in this kernel's epilogue: no separate accumulation pass
-                dx = _nchw(k.conv_dgrad(gi1, w1k, g1, w_crsk=w1t, residual=dxs, res_scale=1.0))
+                dx = nchw(k.conv_dgrad(gi1, w1k, g1, w_crsk=w1t, residual=dxs, res_scale=1.0))
         unprep = k.filter_unprep
         return (dx,
                 unprep(dw1, spec.s1) if dw1 is not None else None, gb1 if need[2] else None,

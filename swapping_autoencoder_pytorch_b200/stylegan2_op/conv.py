@@ -18,7 +18,7 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from .. import backend
-from ..backend import make_geom
+from ..backend import make_geom, nchw, nhwc
 
 
 _data_only = [False]
@@ -39,14 +39,6 @@ def _want_wgrad(ctx, idx):
     ``data_gradients_only()`` (R1's first backward needs the data gradient only; the weight gradient would be computed,
     recorded and thrown away — one forward-equivalent of tensor work per convolution)"""
     return ctx.needs_input_grad[idx] and not (_data_only[0] and torch.is_grad_enabled())
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2)
 
 
 def _impl(g):
@@ -134,7 +126,7 @@ class _ConvFprop(Function):
     def forward(ctx, x, w, wt, g):
         ctx.g = g
         ctx.save_for_backward(x, w, wt)
-        return _nchw(backend.kernels().conv_fprop(_nhwc(x), w.contiguous(), g, impl=_impl(g), prepared=wt is not None))
+        return nchw(backend.kernels().conv_fprop(nhwc(x), w.contiguous(), g, impl=_impl(g), prepared=wt is not None))
 
     @staticmethod
     def backward(ctx, dy):
@@ -151,7 +143,7 @@ class _ConvDgrad(Function):
     def forward(ctx, dy, w, wt, g):
         ctx.g = g
         ctx.save_for_backward(dy, w, wt)
-        return _nchw(backend.kernels().conv_dgrad(_nhwc(dy), w.contiguous(), g, impl=_impl(g), w_crsk=wt))
+        return nchw(backend.kernels().conv_dgrad(nhwc(dy), w.contiguous(), g, impl=_impl(g), w_crsk=wt))
 
     @staticmethod
     def backward(ctx, ddx):
@@ -168,7 +160,7 @@ class _ConvWgrad(Function):
     def forward(ctx, dy, x, g):
         ctx.g = g
         ctx.save_for_backward(dy, x)
-        return backend.kernels().conv_wgrad(_nhwc(dy), _nhwc(x), g, impl=_impl(g))
+        return backend.kernels().conv_wgrad(nhwc(dy), nhwc(x), g, impl=_impl(g))
 
     @staticmethod
     def backward(ctx, ddw):
@@ -186,9 +178,9 @@ class _ConvBiasAct(Function):
 
     @staticmethod
     def forward(ctx, x, w, wt, bias, g, negative_slope, gain):
-        y = backend.kernels().conv_fprop(_nhwc(x), w.contiguous(), g, impl=_impl(g), prepared=wt is not None,
+        y = backend.kernels().conv_fprop(nhwc(x), w.contiguous(), g, impl=_impl(g), prepared=wt is not None,
                                          bias=bias.contiguous(), act=3, alpha=negative_slope, gain=gain)
-        out = _nchw(y)
+        out = nchw(y)
         ctx.g, ctx.cfg, ctx.act_mask = g, (negative_slope, gain), backend.act_mask_of(y)
         ctx.save_for_backward(x, w, wt, out)
         return out
@@ -213,10 +205,10 @@ class _ConvNoiseBiasAct(Function):
     @staticmethod
     def forward(ctx, x, w, wt, noise, noise_weight, bias, g, negative_slope, gain):
         noise_flat = noise.reshape(-1).contiguous()
-        y = backend.kernels().conv_fprop(_nhwc(x), w.contiguous(), g, prepared=wt is not None, bias=bias.contiguous(),
+        y = backend.kernels().conv_fprop(nhwc(x), w.contiguous(), g, prepared=wt is not None, bias=bias.contiguous(),
                                          act=3, alpha=negative_slope, gain=gain, noise=noise_flat,
                                          noise_weight=noise_weight.contiguous())
-        out = _nchw(y)
+        out = nchw(y)
         ctx.g, ctx.cfg, ctx.act_mask = g, (negative_slope, gain, tuple(noise.shape)), backend.act_mask_of(y)
         ctx.save_for_backward(x, w, wt, out, noise_flat, noise_weight)
         return out
@@ -227,10 +219,10 @@ class _ConvNoiseBiasAct(Function):
         x, w, wt, out, noise_flat, noise_weight = ctx.saved_tensors
         negative_slope, gain, noise_shape = ctx.cfg
         k = backend.kernels()
-        gi, gb, gnw = k.bias_act_backward(_nhwc(dy), _nhwc(out), negative_slope, gain, want_bias=True, noise=noise_flat,
+        gi, gb, gnw = k.bias_act_backward(nhwc(dy), nhwc(out), negative_slope, gain, want_bias=True, noise=noise_flat,
                                           mask=ctx.act_mask)
-        dx = _nchw(k.conv_dgrad(gi, w.contiguous(), ctx.g, w_crsk=wt)) if ctx.needs_input_grad[0] else None
-        dw = k.conv_wgrad(gi, _nhwc(x), ctx.g) if ctx.needs_input_grad[1] else None
+        dx = nchw(k.conv_dgrad(gi, w.contiguous(), ctx.g, w_crsk=wt)) if ctx.needs_input_grad[0] else None
+        dw = k.conv_wgrad(gi, nhwc(x), ctx.g) if ctx.needs_input_grad[1] else None
         g_noise = None
         if ctx.needs_input_grad[3]:
             g_noise = (gi.sum(dim=3) * noise_weight).reshape(noise_shape)
@@ -246,8 +238,8 @@ class _ConvResidual(Function):
     def forward(ctx, x, w, wt, res, g, scale):
         ctx.g, ctx.scale = g, scale
         ctx.save_for_backward(x, w, wt)
-        return _nchw(backend.kernels().conv_fprop(_nhwc(x), w.contiguous(), g, prepared=wt is not None, residual=_nhwc(res),
-                                                 res_scale=scale))
+        return nchw(backend.kernels().conv_fprop(nhwc(x), w.contiguous(), g, prepared=wt is not None, residual=nhwc(res),
+                                                res_scale=scale))
 
     @staticmethod
     def backward(ctx, dy):
@@ -266,7 +258,7 @@ class _PadChannels(Function):
     @staticmethod
     def forward(ctx, x, c_out):
         ctx.c_in = x.shape[1]
-        return _nchw(backend.kernels().pad_channels(x, c_out))
+        return nchw(backend.kernels().pad_channels(x, c_out))
 
     @staticmethod
     def backward(ctx, dy):
@@ -446,14 +438,14 @@ class _Modulate(Function):
     @staticmethod
     def forward(ctx, x, s):
         ctx.save_for_backward(x, s)
-        return _nchw(backend.kernels().modulate(_nhwc(x), s.contiguous()))
+        return nchw(backend.kernels().modulate(nhwc(x), s.contiguous()))
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dy):
         x, s = ctx.saved_tensors
-        dx, ds = backend.kernels().modulate_backward(_nhwc(dy), _nhwc(x), s.contiguous())
-        return _nchw(dx), ds
+        dx, ds = backend.kernels().modulate_backward(nhwc(dy), nhwc(x), s.contiguous())
+        return nchw(dx), ds
 
 
 def modulate(x, s):
@@ -472,7 +464,7 @@ class _ModulatedConv(Function):
     @staticmethod
     def forward(ctx, x, s, w, g, noise, noise_weight, bias, negative_slope, gain):
         k = backend.kernels()
-        xh, sc = _nhwc(x), s.contiguous()
+        xh, sc = nhwc(x), s.contiguous()
         w_n, _ = k.filter_modulate(w.contiguous(), sc, want_krsc=True, want_crsk=False)
         act = bias is not None
         epi = {}
@@ -486,7 +478,7 @@ class _ModulatedConv(Function):
         ctx.act_mask = backend.act_mask_of(out)
         ctx.g, ctx.cfg = g, (act, negative_slope, gain, tuple(noise.shape) if noise is not None else None)
         ctx.save_for_backward(xh, sc, w, out if act else None, noise_flat, noise_weight if noise is not None else None)
-        return _nchw(out)
+        return nchw(out)
 
     @staticmethod
     @once_differentiable
@@ -494,13 +486,13 @@ class _ModulatedConv(Function):
         xh, sc, w, out, noise_flat, noise_weight = ctx.saved_tensors
         act, negative_slope, gain, noise_shape = ctx.cfg
         k = backend.kernels()
-        gi, gb, gnw = _nhwc(dy), None, None
+        gi, gb, gnw = nhwc(dy), None, None
         if act:
             gi, gb, gnw = k.bias_act_backward(gi, out, negative_slope, gain, want_bias=True, noise=noise_flat, mask=ctx.act_mask)
         dx = None
         if ctx.needs_input_grad[0]:
             _, w_nt = k.filter_modulate(w.contiguous(), sc, want_krsc=False, want_crsk=True)
-            dx = _nchw(k.conv_dgrad_per_sample(gi, w_nt, ctx.g))
+            dx = nchw(k.conv_dgrad_per_sample(gi, w_nt, ctx.g))
         dw = ds = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
             dw, ds = k.conv_wgrad_modulated(gi, xh, sc, w.contiguous(), ctx.g)
@@ -542,11 +534,11 @@ class _ToRGB(Function):
 
     @staticmethod
     def forward(ctx, x, s, w, bias, wscale):
-        xh, sc, wc = _nhwc(x), s.contiguous(), w.reshape(3, -1).contiguous()
+        xh, sc, wc = nhwc(x), s.contiguous(), w.reshape(3, -1).contiguous()
         y = backend.kernels().torgb_forward(xh, sc, wc, bias.reshape(-1).contiguous() if bias is not None else None, wscale)
         ctx.save_for_backward(xh, sc, wc)
         ctx.wscale, ctx.w_shape, ctx.bias_shape = wscale, tuple(w.shape), (tuple(bias.shape) if bias is not None else None)
-        return _nchw(y)[:, :3]
+        return nchw(y)[:, :3]
 
     @staticmethod
     @once_differentiable
@@ -561,7 +553,7 @@ class _ToRGB(Function):
             dw = ((gw * sc.unsqueeze(1)).sum(dim=0) * ctx.wscale).reshape(ctx.w_shape)
         if need[3]:
             db = dy.sum(dim=(0, 2, 3)).reshape(ctx.bias_shape)
-        return (_nchw(dx) if dx is not None else None), ds, dw, db, None
+        return (nchw(dx) if dx is not None else None), ds, dw, db, None
 
 
 def torgb(x, s, w, bias, wscale):
@@ -578,7 +570,7 @@ class _AddScale(Function):
         ctx.scale = scale
         k = backend.kernels()
         if a.dim() == 4:
-            return _nchw(k.add_scale(_nhwc(a), _nhwc(b) if b is not None else None, scale))
+            return nchw(k.add_scale(nhwc(a), nhwc(b) if b is not None else None, scale))
         return k.add_scale(a.contiguous(), b.contiguous() if b is not None else None, scale)
 
     @staticmethod
@@ -598,7 +590,7 @@ class _ReflectPad(Function):
     @staticmethod
     def forward(ctx, x, pads):
         ctx.pads = pads
-        return _nchw(backend.kernels().reflect_pad(_nhwc(x), pads))
+        return nchw(backend.kernels().reflect_pad(nhwc(x), pads))
 
     @staticmethod
     def backward(ctx, dy):
@@ -609,7 +601,7 @@ class _ReflectPadAdjoint(Function):
     @staticmethod
     def forward(ctx, dy, pads):
         ctx.pads = pads
-        return _nchw(backend.kernels().reflect_pad_backward(_nhwc(dy), pads))
+        return nchw(backend.kernels().reflect_pad_backward(nhwc(dy), pads))
 
     @staticmethod
     def backward(ctx, ddx):
@@ -631,18 +623,18 @@ class _Upsample2xAddScale(Function):
     @staticmethod
     def forward(ctx, skip, res, scale):
         ctx.scale = scale
-        return _nchw(backend.kernels().upsample2x_add_scale(_nhwc(skip), _nhwc(res), scale))
+        return nchw(backend.kernels().upsample2x_add_scale(nhwc(skip), nhwc(res), scale))
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dy):
         k = backend.kernels()
-        g = _nhwc(dy)
-        d_skip = _nchw(k.upsample2x_backward(g, ctx.scale)) if ctx.needs_input_grad[0] else None
+        g = nhwc(dy)
+        d_skip = nchw(k.upsample2x_backward(g, ctx.scale)) if ctx.needs_input_grad[0] else None
         if ctx.scale == 1.0:
             d_res = dy if ctx.needs_input_grad[1] else None
         else:
-            d_res = _nchw(k.add_scale(g, None, ctx.scale)) if ctx.needs_input_grad[1] else None
+            d_res = nchw(k.add_scale(g, None, ctx.scale)) if ctx.needs_input_grad[1] else None
         return d_skip, d_res, None
 
 

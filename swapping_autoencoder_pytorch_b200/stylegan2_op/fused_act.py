@@ -10,15 +10,16 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from .. import backend
+from ..backend import nchw, nhwc
 
 
 def _cl(t):
-    """channel dim (1) moved last, contiguous: physical layout the kernels use"""
-    return t.movedim(1, -1).contiguous() if t.dim() > 2 else t.contiguous()
+    """the kernels' layout of an activation: NHWC for a feature map, a [B, C] matrix as it is"""
+    return nhwc(t) if t.dim() > 2 else t.contiguous()
 
 
 def _uncl(t):
-    return t.movedim(-1, 1) if t.dim() > 2 else t
+    return nchw(t) if t.dim() > 2 else t
 
 
 class FusedLeakyReLUFunctionBackward(Function):

@@ -10,14 +10,7 @@ import torch
 from torch.autograd import Function
 
 from .. import backend
-
-
-def _nhwc(t):
-    return t.permute(0, 2, 3, 1).contiguous()
-
-
-def _nchw(t):
-    return t.permute(0, 3, 1, 2)
+from ..backend import nchw, nhwc
 
 
 def _out_extent(n_in, up, down, p0, p1, k):
@@ -30,20 +23,20 @@ class UpFirDn2dBackward(Function):
     @staticmethod
     def forward(ctx, grad_output, kernel, grad_kernel, up, down, pad, g_pad, in_size, out_size, taps=None):
         gx0, gx1, gy0, gy1 = g_pad
-        g = backend.kernels().upfirdn2d(_nhwc(grad_output), grad_kernel, down[0], down[1], up[0], up[1],
+        g = backend.kernels().upfirdn2d(nhwc(grad_output), grad_kernel, down[0], down[1], up[0], up[1],
                                         gx0, gx1, gy0, gy1, taps=_flip_taps(taps))
         # the adjoint can come out larger than the input when the forward dropped trailing rows; never here
         assert g.shape[1] == in_size[2] and g.shape[2] == in_size[3], (tuple(g.shape), tuple(in_size))
         ctx.save_for_backward(kernel)
         ctx.cfg = (up, down, pad, taps)
-        return _nchw(g)
+        return nchw(g)
 
     @staticmethod
     def backward(ctx, gradgrad_input):
         kernel, = ctx.saved_tensors
         up, down, pad, taps = ctx.cfg
-        gg = backend.kernels().upfirdn2d(_nhwc(gradgrad_input), kernel, up[0], up[1], down[0], down[1], *pad, taps=taps)
-        return _nchw(gg), None, None, None, None, None, None, None, None, None
+        gg = backend.kernels().upfirdn2d(nhwc(gradgrad_input), kernel, up[0], up[1], down[0], down[1], *pad, taps=taps)
+        return nchw(gg), None, None, None, None, None, None, None, None, None
 
 
 class UpFirDn2d(Function):
@@ -65,8 +58,8 @@ class UpFirDn2d(Function):
                  in_h * up_y - out_h * down_y + py0 - up_y + 1)
         ctx.save_for_backward(kernel, torch.flip(kernel, [0, 1]))
         ctx.cfg = (up, down, pad, g_pad, tuple(input.shape), (out_h, out_w), taps)
-        out = backend.kernels().upfirdn2d(_nhwc(input), kernel, up_x, up_y, down_x, down_y, px0, px1, py0, py1, taps=taps)
-        return _nchw(out)
+        out = backend.kernels().upfirdn2d(nhwc(input), kernel, up_x, up_y, down_x, down_y, px0, px1, py0, py1, taps=taps)
+        return nchw(out)
 
     @staticmethod
     def backward(ctx, grad_output):
