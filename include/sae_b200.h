@@ -31,7 +31,7 @@ extern "C" {
 #define SAE_E_UNSUPPORTED  -3   /* valid request this build has no kernel for                */
 
 /* ABI version of this header; bumped on any signature change. */
-#define SAE_ABI_VERSION 16
+#define SAE_ABI_VERSION 17
 int         sae_abi_version(void);
 const char* sae_last_error(void);
 /* number of kernels launched by this library in the calling process since load
@@ -263,6 +263,15 @@ int sae_bucket_pack(const float* const* ptrs, const int64_t* offsets, const int6
                     float* bucket, int64_t total, void* stream);
 int sae_bucket_unpack(float* const* ptrs, const int64_t* offsets, const int64_t* sizes, int n,
                       const float* bucket, int64_t total, float scale, void* stream);
+/* Gradient accumulation (ABI 17; SwappingAutoencoderOptimizer with opt.micro_batches > 1): one optimizer update from the
+ * summed gradients of several micro-batches.  Micro-batch 0 is copied in with sae_bucket_pack; sae_bucket_accumulate adds
+ * every later one in the same layout:  bucket[offsets[t] + i] += ptrs[t][i]  for i < sizes[t], t < n.  A NULL pointer skips
+ * its tensor.  Each element is one round-to-nearest fp32 add (bitwise a + b), no atomics: the result is independent of the
+ * schedule and deterministic mode needs no twin.  Gradients of any alignment (16-byte aligned ones are read as float4);
+ * 64-bit indexing; n <= 65535 (SAE_E_UNSUPPORTED above).  Null tables or bucket with n > 0, n < 0 or total < 0:
+ * SAE_E_INVALID; n == 0: SAE_OK, nothing launched. */
+int sae_bucket_accumulate(const float* const* ptrs, const int64_t* offsets, const int64_t* sizes, int n,
+                          float* bucket, int64_t total, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Style-modulated convolution WITHOUT a modulated copy of the activation (SURVEY.md §8 a5).

@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsae_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
 
-SAE_ABI_VERSION = 16
+SAE_ABI_VERSION = 17
 SAE_E_UNSUPPORTED = -3        # a valid request no kernel of this build takes (header: SAE_E_*)
 
 c_float_p = ctypes.c_void_p   # raw device pointers travel as integers
@@ -99,6 +99,8 @@ SIGNATURES = {
                                        ctypes.c_int64, c_stream]),
     "sae_bucket_unpack": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, c_float_p,
                                          ctypes.c_int64, ctypes.c_float, c_stream]),
+    "sae_bucket_accumulate": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, c_float_p,
+                                             ctypes.c_int64, c_stream]),
     "sae_filter_modulate": (ctypes.c_int, [c_float_p] * 4 + [ctypes.c_int] * 6 + [c_stream]),
     "sae_conv2d_query_modulated": (ctypes.c_int, [ctypes.POINTER(ConvGeom)]),
     "sae_conv2d_fprop_per_sample": (ctypes.c_int, [c_float_p, c_float_p, c_float_p, ctypes.POINTER(ConvGeom),

@@ -517,6 +517,11 @@ class CudaKernels:
         self._launch(bucket.device, "sae_bucket_unpack", _ptr(ptrs), _ptr(offsets), _ptr(sizes), n, _ptr(bucket), bucket.numel(),
                      scale)
 
+    def bucket_accumulate(self, ptrs, offsets, sizes, n, bucket):
+        """bucket[offsets[t] + i] += tensor t of the pointer table ``ptrs`` (the layout of ``bucket_pack``; NULL: skipped)"""
+        self._launch(bucket.device, "sae_bucket_accumulate", _ptr(ptrs), _ptr(offsets), _ptr(sizes), n, _ptr(bucket),
+                     bucket.numel())
+
 
     # ----------------------------------------------------------------- Adam
     def adam_step(self, params, grads, offsets, sizes, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, grad_scale, cache,

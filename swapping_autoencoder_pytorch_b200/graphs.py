@@ -13,6 +13,9 @@ images copied into a static input buffer.
 * Random draws (NoiseInjection, crop windows) use torch's graph-safe Philox generator: every replay draws fresh numbers.
 * Data parallel (world > 1): the graph holds forward + backward only; the gradient all-reduce (``parallel.py``) and the
   Adam step run eagerly after the replay on the graph's static gradient buffers — no NCCL call is captured.
+* Gradient accumulation (opt.micro_batches = k > 1): the graph holds one micro-batch's forward + backward, replayed k times
+  per update; the trainer packs (first replay) or adds (later ones) the static gradient buffers into the flat bucket after
+  each replay and issues the exchange, the guard scan and Adam eagerly after the last.  One graph per kind and k.
 * A body that fails to capture falls back to eager execution for the rest of the run (``self.disabled`` holds why).
 """
 import gc
@@ -30,7 +33,8 @@ class HalfStepGraphs:
         self.trainer = trainer
         self.warmup = warmup
         self.calls = {}
-        # (kind, input shape, kernel precision, deterministic, non-finite guard) -> (graph, static_input, static_outputs, launches, ...)
+        # (kind, input shape, kernel precision, deterministic, non-finite guard[, micro-batches when > 1]) -> (graph, static_input,
+        # static_outputs, launches, ...)
         self.captured = {}
         self.pool = None
         self.stream = None             # side stream shared by the eager warm-up calls and every capture (see _side)
@@ -94,9 +98,12 @@ class HalfStepGraphs:
             pass
         torch.cuda.synchronize()
 
-    def run(self, kind, body, images):
+    def run(self, kind, body, images, micro_batches=1):
+        """micro_batches > 1: ``images`` is one micro-batch of an accumulated update; the body runs (and is captured) with
+        step=False and nothing follows the replay — the caller accumulates the gradients and steps (optimizer._run)"""
+        step = micro_batches == 1
         if self.disabled is not None or not self.enabled:
-            return body(images)
+            return body(images) if step else body(images, step=False)
         # a graph records the kernels of one precision mode (backend.CudaKernels.precision): switching the mode captures new
         # graphs, after warm-up calls of their own (the other mode's kernels initialise lazily, outside any capture).  The same
         # holds for the deterministic mode (backend.CudaKernels.deterministic_mode()), which records other kernels, and for the
@@ -105,13 +112,14 @@ class HalfStepGraphs:
         precision = getattr(k, "precision", "tf32")
         det = bool(getattr(k, "deterministic_mode", lambda: False)())
         guard = self.trainer.nonfinite_guard_on()
-        n = self.calls.get((kind, precision, det, guard), 0)
-        self.calls[(kind, precision, det, guard)] = n + 1
-        key = (kind, tuple(images.shape), precision, det, guard)
+        extra = () if step else (micro_batches,)          # k = 1 keeps the keys it always had
+        n = self.calls.get((kind, precision, det, guard) + extra, 0)
+        self.calls[(kind, precision, det, guard) + extra] = n + 1
+        key = (kind, tuple(images.shape), precision, det, guard) + extra
         hit = self.captured.get(key)
         if hit is None:
             if n < self.warmup:
-                return self._side(lambda: body(images))
+                return self._side(lambda: body(images) if step else body(images, step=False))
             try:
                 try:
                     hit = self._capture(key, body, images, self.nccl_in_graph)
@@ -126,7 +134,7 @@ class HalfStepGraphs:
                     hit = self._capture(key, body, images, False)
             except Exception as e:      # noqa: BLE001 — any capture failure means "run eagerly", never "stop training"
                 self._give_up(kind, e)
-                return body(images)
+                return body(images) if step else body(images, step=False)
         graph, static_in, outputs, launches, grads, tail_captured = hit
         # host-side state the eager body would have left behind: which group is trainable, and which gradient buffers
         # the parameters point at (every graph owns its own static set)
@@ -143,7 +151,7 @@ class HalfStepGraphs:
         self.replayed_launches += launches
         if ev is not None:
             ev[1].record()
-        if self._world() > 1 and not tail_captured:
+        if step and self._world() > 1 and not tail_captured:
             self._tail(kind)
         if ev is not None:
             ev[2].record()
@@ -187,6 +195,8 @@ class HalfStepGraphs:
     def _capture(self, key, body, images, with_tail=False):
         kind = key[0]
         world = self._world()
+        step = len(key) == 5            # a sixth element is the micro-batch count of an accumulated update
+        with_tail = with_tail and step
         wrapper = self._wrapper()
         static_in = torch.empty_like(images).requires_grad_(False)
         with torch.no_grad():
@@ -211,7 +221,7 @@ class HalfStepGraphs:
         gc.disable()
         try:
             with torch.cuda.graph(graph, pool=self.pool, stream=self.stream):
-                outputs = body(static_in, step=(world == 1))
+                outputs = body(static_in, step=(world == 1 and step))
                 if world > 1 and with_tail:
                     self._tail(kind)
         finally:

@@ -134,6 +134,9 @@ class SwappingAutoencoderOptimizer:
         parser.add_argument("--beta2", default=0.99, type=float)
         parser.add_argument("--R1_once_every", default=16, type=int,
                             help="lazy R1 regularization: the R1 loss is computed once every this many D iterations")
+        parser.add_argument("--micro_batches", default=1, type=int,
+                            help="gradient accumulation (extension): split each rank's batch into this many micro-batches and "
+                                 "make one Adam update from their summed gradients")
         return parser
 
     def __init__(self, model):
@@ -200,13 +203,17 @@ class SwappingAutoencoderOptimizer:
         params = self.Gparams if kind == "G" else self.Dparams
         return {names[id(p)]: c for p, c in zip(params, g.report.tolist()) if c}
 
-    def exchange_and_step(self, optimizer, params, kind=None):
+    def exchange_and_step(self, optimizer, params, kind=None, micro_batches=1):
         """optimizer step of one half-step; with more than one rank: pack -> all-reduce (SUM) -> Adam reading the bucket.
         With ``opt.skip_nonfinite_steps`` the gradients Adam reads (the reduced bucket with more than one rank: the same bytes
-        on every rank) are scanned first and a non-finite one drops the update of the half-step ``kind``."""
+        on every rank) are scanned first and a non-finite one drops the update of the half-step ``kind``.
+        micro_batches > 1: the gradients were summed into the bucket by ``accumulate_to_bucket`` after every micro-batch; one
+        all-reduce (world > 1), one scan, one Adam update reading the bucket with grad_scale = 1 / (micro_batches * world)."""
         guard = self.nonfinite_guard(kind) if kind is not None and self.nonfinite_guard_on() else None
         kw = {} if guard is None else {"guard": guard}
-        if self.world > 1:
+        if micro_batches > 1:
+            optimizer.step(grads=self.model.reduce_accumulated(), grad_scale=1.0 / (micro_batches * self.world), **kw)
+        elif self.world > 1:
             optimizer.step(grads=self.model.reduce_to_bucket(params), grad_scale=1.0 / self.world, **kw)
         else:
             optimizer.step(**kw)
@@ -228,6 +235,7 @@ class SwappingAutoencoderOptimizer:
         """One half-step.  The toggle returns "generator" first, which selects the *discriminator* update
         (reference :59-65) — strict D, G, D, G alternation starting with D."""
         images = self.prepare_images(data_i)
+        self.split_micro_batches(images)            # a batch that does not split raises before the schedule moves
         if self.toggle_training_mode() == "generator":
             losses = self.train_discriminator_one_step(images)
         else:
@@ -269,12 +277,59 @@ class SwappingAutoencoderOptimizer:
             self.exchange_and_step(self.optimizer_D, self.Dparams, kind="R1")
         return r1_losses
 
+    # ------------------------------------------------------------------ gradient accumulation (extension, opt.micro_batches)
+    def micro_batches(self):
+        return getattr(self.opt, "micro_batches", 1)
+
+    def split_micro_batches(self, images):
+        """the rank's images [B, ...] as opt.micro_batches consecutive slices of B / k images along dim 0; ValueError unless
+        k divides B into even micro-batches of at least 2 images (``swap`` pairs images).  k = 1: [images], unchecked."""
+        k = self.micro_batches()
+        if k == 1:
+            return [images]
+        if not isinstance(k, int) or isinstance(k, bool) or k < 1:
+            raise ValueError("opt.micro_batches must be a positive integer, got %r" % (k,))
+        n = images.shape[0]
+        if n % k != 0 or (n // k) % 2 != 0 or n // k < 2:
+            raise ValueError("a batch of %d images does not split into %d micro-batches of an even number of images" % (n, k))
+        b = n // k
+        return [images[j * b:(j + 1) * b] for j in range(k)]
+
+    @staticmethod
+    def _mean_outputs(parts):
+        """one body's outputs over the micro-batches of an update: every value the mean of its k micro-batch means, formed on
+        the device; the codes ("_sp", "_gl") concatenated, so they keep the full batch's shape"""
+        out = {}
+        for key in parts[0]:
+            vals = [p[key] for p in parts]
+            out[key] = torch.cat(vals) if key in ("_sp", "_gl") else torch.stack(vals).mean()
+        return out
+
     def _run(self, kind, images):
-        """Eager execution of one body, or — with ``opt.cuda_graphs`` on a CUDA device — replay of its CUDA graph."""
+        """Eager execution of one body, or — with ``opt.cuda_graphs`` on a CUDA device — replay of its CUDA graph.
+        With opt.micro_batches = k > 1: the body once per micro-batch with step=False (eager or replayed), its gradients
+        summed into the flat bucket after each, then one exchange and one Adam update (exchange_and_step)."""
         body = {"G": self._generator_body, "D": self._discriminator_body, "R1": self._r1_body}[kind]
-        if self.graphs is not None and images.is_cuda:
-            return self.graphs.run(kind, body, images)
-        return body(images)
+        chunks = self.split_micro_batches(images)
+        k = len(chunks)
+        if k == 1:
+            if self.graphs is not None and images.is_cuda:
+                return self.graphs.run(kind, body, images)
+            return body(images)
+        params = self.Gparams if kind == "G" else self.Dparams
+        parts = []
+        for j, chunk in enumerate(chunks):
+            if self.graphs is not None and chunk.is_cuda:
+                out = self.graphs.run(kind, body, chunk, micro_batches=k)
+            else:
+                out = body(chunk, step=False)
+            self.model.accumulate_to_bucket(params, j)
+            # a replay's outputs are the graph's static buffers, which the next replay overwrites: reduce / copy them now
+            with torch.no_grad():
+                parts.append({key: (v.detach().clone() if key in ("_sp", "_gl") else v.detach().mean())
+                              for key, v in out.items() if torch.is_tensor(v)})
+        self.exchange_and_step(self.optimizer_G if kind == "G" else self.optimizer_D, params, kind=kind, micro_batches=k)
+        return self._mean_outputs(parts)
 
     def train_generator_one_step(self, images):
         return self._run("G", images)
@@ -285,6 +340,10 @@ class SwappingAutoencoderOptimizer:
             return {}
         self.discriminator_iter_counter += 1
         d_losses = dict(self._run("D", images))
+        micro = self.micro_batches()
+        if micro > 1:
+            # compute_discriminator_losses advanced the model's iteration buffer once per micro-batch; it counts D updates
+            getattr(self.model, "singlegpu_model", self.model).num_discriminator_iters.sub_(micro - 1)
         self.previous_sp, self.previous_gl = d_losses.pop("_sp"), d_losses.pop("_gl")
         d_metrics = {k[len("_metric:"):]: d_losses.pop(k) for k in list(d_losses) if k.startswith("_metric:")}
 

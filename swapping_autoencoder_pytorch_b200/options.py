@@ -41,6 +41,10 @@ def default_options(**overrides):
         # or an Inf (parameters, moments and step counts stay bitwise unchanged); nonfinite_steps() / nonfinite_report() tell
         # how often and where (optimizer.NonfiniteGuard)
         skip_nonfinite_steps=False,
+        # extension: gradient accumulation — each rank's batch is split into this many micro-batches, run one after the other,
+        # and one Adam update is made from their summed gradients, so the global batch no longer has to fit one pass per GPU
+        # (SwappingAutoencoderOptimizer.split_micro_batches; INTEGRATION.md §2e)
+        micro_batches=1,
     )
     for k, v in overrides.items():
         setattr(opt, k, v)

@@ -64,8 +64,9 @@ class GradientBucket:
         if self.flat is None or self.flat.numel() < total:
             self.flat = torch.zeros(total, dtype=torch.float32, device=self.device)
 
-    def pack_all_reduce(self, grads):
-        """SUM over ranks of the given gradient tensors, left in the flat bucket; returns one bucket view per gradient"""
+    def fill(self, grads, micro_batch=0):
+        """copy the given gradient tensors into the flat bucket (micro_batch 0: sae_bucket_pack), or add them to what it holds
+        (a later micro-batch of the same update, same tensors: sae_bucket_accumulate); returns one bucket view per gradient"""
         offsets_t, sizes_t, total, offsets = self._layout(grads)
         self.reserve(total)
         flat = self.flat[:total]
@@ -73,9 +74,17 @@ class GradientBucket:
             self.tables = backend.PointerTables(max(len(grads), 1024), self.device)
         ptrs = self.tables.get(tuple(g.data_ptr() for g in grads))
         k = backend.kernels()
-        k.bucket_pack(ptrs, offsets_t, sizes_t, len(grads), flat)
-        dist.all_reduce(flat)
+        if micro_batch == 0:
+            k.bucket_pack(ptrs, offsets_t, sizes_t, len(grads), flat)
+        else:
+            k.bucket_accumulate(ptrs, offsets_t, sizes_t, len(grads), flat)
         return [flat[o:o + g.numel()].view_as(g) for o, g in zip(offsets, grads)], (ptrs, offsets_t, sizes_t, flat)
+
+    def pack_all_reduce(self, grads):
+        """SUM over ranks of the given gradient tensors, left in the flat bucket; returns one bucket view per gradient"""
+        views, info = self.fill(grads)
+        dist.all_reduce(info[3])
+        return views, info
 
     def all_reduce_mean(self, grads, world):
         if not grads:
@@ -110,6 +119,7 @@ class MultiGPUModelWrapper:
         # callback, which averages INTO p.grad for a stock optimizer, is then not queued
         self.defer_to_optimizer = False
         self._bucket = GradientBucket(self.device)
+        self._accumulated = None     # (flat, views, which params have a gradient) of the update being accumulated
         model(command="per_gpu_initialize")
         if self.world > 1:
             with torch.no_grad():
@@ -156,6 +166,44 @@ class MultiGPUModelWrapper:
             views, _ = self._bucket.pack_all_reduce([p.grad for p in present])
         it = iter(views)
         return [next(it) if p.grad is not None else None for p in params]
+
+    def accumulate_to_bucket(self, params, micro_batch):
+        """Gradient accumulation (opt.micro_batches > 1), called after each micro-batch's backward: micro-batch 0 packs the
+        existing gradients of ``params`` into the flat bucket, every later one adds its gradients (the same tensors) to it, in
+        micro-batch order.  At world size 1 the bucket is only this sum; D and G share it, as their updates never overlap.
+        ``reduce_accumulated`` ends the update.  On a CPU device (the gloo tests) the same sums are formed in torch."""
+        present = [p.grad is not None for p in params]
+        grads = [p.grad for p in params if p.grad is not None]
+        if micro_batch == 0:
+            self._accumulated = None
+        elif self._accumulated is None or self._accumulated[2] != present:
+            raise RuntimeError("accumulate_to_bucket: micro-batch %d has other gradients than micro-batch 0" % micro_batch)
+        if not grads:
+            self._accumulated = (None, [], present)
+            return
+        if self.device.type != "cuda":
+            flat = torch.cat([g.reshape(-1) for g in grads])
+            if micro_batch == 0:
+                views, o = [], 0
+                for g in grads:
+                    views.append(flat[o:o + g.numel()].view_as(g))
+                    o += g.numel()
+                self._accumulated = (flat, views, present)
+            else:
+                self._accumulated[0].add_(flat)
+            return
+        views, (_, _, _, flat) = self._bucket.fill(grads, micro_batch)
+        self._accumulated = (flat, views, present)
+
+    def reduce_accumulated(self):
+        """the summed gradients of the update's micro-batches, all-reduced (SUM) once over the ranks when world > 1: a list
+        aligned with the ``params`` given to ``accumulate_to_bucket`` of bucket views (None where a parameter has no gradient)"""
+        flat, views, present = self._accumulated
+        self._accumulated = None
+        if self.world > 1 and flat is not None:
+            dist.all_reduce(flat)
+        it = iter(views)
+        return [next(it) if has else None for has in present]
 
     def get_parameters_for_mode(self, mode):
         return self.singlegpu_model.get_parameters_for_mode(mode)
