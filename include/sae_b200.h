@@ -31,7 +31,7 @@ extern "C" {
 #define SAE_E_UNSUPPORTED  -3   /* valid request this build has no kernel for                */
 
 /* ABI version of this header; bumped on any signature change. */
-#define SAE_ABI_VERSION 17
+#define SAE_ABI_VERSION 18
 int         sae_abi_version(void);
 const char* sae_last_error(void);
 /* number of kernels launched by this library in the calling process since load
@@ -336,6 +336,24 @@ int sae_nonfinite_count(const float* const* ptrs, const int64_t* sizes, int n, u
 int sae_adam_step_guarded(float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets, const int64_t* sizes,
                           int n, float* exp_avg, float* exp_avg_sq, float* steps, float lr, float beta1, float beta2,
                           float eps, float grad_scale, const unsigned long long* skip, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Exponential moving average of the weights (ABI 18; SwappingAutoencoderOptimizer with opt.ema_kimg > 0, INTEGRATION §2f).
+ *   shadow[offsets[t] + i] = fmaf(beta, shadow[offsets[t] + i] - p_ptrs[t][i], p_ptrs[t][i])   for i < sizes[t], every
+ *   non-NULL p_ptrs[t], t < n;  then *updates += 1.
+ * beta is formed on the device, in fp64 and rounded to fp32 once, from t = *updates (the averaging updates already made):
+ *   h = half_life_images, or min(half_life_images, t * batch_images * rampup) when rampup > 0;  beta = 0.5^(batch_images /
+ *   max(h, 1e-8)).  With a ramp, t = 0 gives beta = 0: the first update copies the parameters.  So one launch sequence (one
+ *   captured graph) serves every step of the ramp.  p_ptrs / offsets / sizes: device arrays as for sae_adam_step (the shadow
+ *   takes the layout of the moments); updates: one device int64.  skip (may be NULL): when *skip != 0 (read by the kernels,
+ *   as in sae_adam_step_guarded) the shadow and *updates are left bitwise unchanged.  Elementwise, no atomics: deterministic
+ *   mode needs no twin.  Parameters of any alignment (16-byte aligned ones are read as float4); 64-bit indexing.  Null
+ *   pointers (skip aside), total < 0, n outside [0, 65535], half_life_images <= 0, rampup < 0 or batch_images <= 0 (NaN
+ *   included): SAE_E_INVALID before any CUDA call.  n == 0 only advances *updates.
+ * ------------------------------------------------------------------------------------------ */
+int sae_ema_update(const float* const* p_ptrs, const int64_t* offsets, const int64_t* sizes, int n, float* shadow,
+                   int64_t total, int64_t* updates, float batch_images, float half_life_images, float rampup,
+                   const unsigned long long* skip, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Random-crop resampler of the patch discriminator (SURVEY.md §8 f1).  Replaces

@@ -557,6 +557,20 @@ class CudaKernels:
         tab = cache.get(tuple(0 if t is None else t.data_ptr() for t in tensors))
         self._launch(counts.device, "sae_nonfinite_count", _ptr(tab), _ptr(sizes), len(tensors), _ptr(counts))
 
+    def ema_update(self, params, offsets, sizes, shadow, updates, batch_images, half_life_images, rampup, cache, skip=None):
+        """One averaging update of the flat ``shadow`` towards ``params`` (sae_ema_update; INTEGRATION §2f), then
+        ``updates += 1``.  offsets / sizes: device int64 tensors locating each parameter's segment of ``shadow`` (the layout of
+        ``adam_step``'s moments); updates: one-element device int64 tensor, the averaging updates already made, from which the
+        kernel forms beta; cache: the caller's ``PointerTables``.  skip: optional one-element device int64 tensor; a non-zero
+        value leaves shadow and updates unchanged."""
+        _need_cuda(shadow, *params)
+        _need_int64(updates)
+        if skip is not None:
+            _need_int64(skip)
+        p_tab = cache.get(tuple(p.data_ptr() for p in params))
+        self._launch(shadow.device, "sae_ema_update", _ptr(p_tab), _ptr(offsets), _ptr(sizes), len(params), _ptr(shadow),
+                     shadow.numel(), _ptr(updates), float(batch_images), float(half_life_images), float(rampup), _ptr(skip))
+
     # ----------------------------------------------------------------- ToRGB
     def torgb_forward(self, x, s, w, bias, wscale):
         """x [N,H,W,C], s [N,C], w [3,C], bias [3] or None -> y [N,H,W,4] (channel 3 zero)"""

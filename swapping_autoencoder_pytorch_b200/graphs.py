@@ -16,6 +16,9 @@ images copied into a static input buffer.
 * Gradient accumulation (opt.micro_batches = k > 1): the graph holds one micro-batch's forward + backward, replayed k times
   per update; the trainer packs (first replay) or adds (later ones) the static gradient buffers into the flat bucket after
   each replay and issues the exchange, the guard scan and Adam eagerly after the last.  One graph per kind and k.
+* Weight averaging (opt.ema_kimg > 0): the averaging update follows the G update's Adam wherever that runs (inside the G
+  graph at world size 1); it forms beta on the device from a counter that lives outside the pool, so one graph serves every
+  step of the ramp.
 * A body that fails to capture falls back to eager execution for the rest of the run (``self.disabled`` holds why).
 """
 import gc
@@ -33,8 +36,8 @@ class HalfStepGraphs:
         self.trainer = trainer
         self.warmup = warmup
         self.calls = {}
-        # (kind, input shape, kernel precision, deterministic, non-finite guard[, micro-batches when > 1]) -> (graph, static_input,
-        # static_outputs, launches, ...)
+        # (kind, input shape, kernel precision, deterministic, non-finite guard[, micro-batches when > 1][, the average's
+        # setting for G when it is on]) -> (graph, static_input, static_outputs, launches, ...)
         self.captured = {}
         self.pool = None
         self.stream = None             # side stream shared by the eager warm-up calls and every capture (see _side)
@@ -61,9 +64,9 @@ class HalfStepGraphs:
     def _optimizer(self, kind):
         return self.trainer.optimizer_G if kind == "G" else self.trainer.optimizer_D
 
-    def _tail(self, kind):
+    def _tail(self, kind, images):
         """world > 1: pack the static gradient buffers, all-reduce, Adam reading the bucket (optimizer.exchange_and_step)"""
-        self.trainer.exchange_and_step(self._optimizer(kind), self._params(kind), kind=kind)
+        self.trainer.exchange_and_step(self._optimizer(kind), self._params(kind), kind=kind, images=images.shape[0])
 
     def _side(self, fn):
         """Run ``fn`` on the capture stream.  The warm-up calls must run where the capture will: autograd remembers
@@ -107,12 +110,15 @@ class HalfStepGraphs:
         # a graph records the kernels of one precision mode (backend.CudaKernels.precision): switching the mode captures new
         # graphs, after warm-up calls of their own (the other mode's kernels initialise lazily, outside any capture).  The same
         # holds for the deterministic mode (backend.CudaKernels.deterministic_mode()), which records other kernels, and for the
-        # non-finite guard (opt.skip_nonfinite_steps), which adds the scan and the guarded update.
+        # non-finite guard (opt.skip_nonfinite_steps), which adds the scan and the guarded update, and for the weight average
+        # (opt.ema_kimg), whose launch the G graph holds.
         k = backend.kernels()
         precision = getattr(k, "precision", "tf32")
         det = bool(getattr(k, "deterministic_mode", lambda: False)())
         guard = self.trainer.nonfinite_guard_on()
         extra = () if step else (micro_batches,)          # k = 1 keeps the keys it always had
+        if kind == "G":
+            extra += self.trainer.ema_key()                # () with the average off
         n = self.calls.get((kind, precision, det, guard) + extra, 0)
         self.calls[(kind, precision, det, guard) + extra] = n + 1
         key = (kind, tuple(images.shape), precision, det, guard) + extra
@@ -122,7 +128,7 @@ class HalfStepGraphs:
                 return self._side(lambda: body(images) if step else body(images, step=False))
             try:
                 try:
-                    hit = self._capture(key, body, images, self.nccl_in_graph)
+                    hit = self._capture(key, body, images, self.nccl_in_graph, step)
                 except Exception as e:      # noqa: BLE001
                     if not (self.nccl_in_graph and self._world() > 1):
                         raise
@@ -131,7 +137,7 @@ class HalfStepGraphs:
                     self.nccl_in_graph = False
                     self.nccl_capture_error = "%s: %s" % (type(e).__name__, (str(e).splitlines() or ["?"])[0][:200])
                     self._recover()
-                    hit = self._capture(key, body, images, False)
+                    hit = self._capture(key, body, images, False, step)
             except Exception as e:      # noqa: BLE001 — any capture failure means "run eagerly", never "stop training"
                 self._give_up(kind, e)
                 return body(images) if step else body(images, step=False)
@@ -152,7 +158,7 @@ class HalfStepGraphs:
         if ev is not None:
             ev[1].record()
         if step and self._world() > 1 and not tail_captured:
-            self._tail(kind)
+            self._tail(kind, images)
         if ev is not None:
             ev[2].record()
             self.phase_events.append((kind, ev))
@@ -192,10 +198,10 @@ class HalfStepGraphs:
                 self.run(kind, body, images)
         torch.cuda.synchronize()
 
-    def _capture(self, key, body, images, with_tail=False):
+    def _capture(self, key, body, images, with_tail=False, step=True):
+        """step=False: one micro-batch of an accumulated update, captured without the optimizer step"""
         kind = key[0]
         world = self._world()
-        step = len(key) == 5            # a sixth element is the micro-batch count of an accumulated update
         with_tail = with_tail and step
         wrapper = self._wrapper()
         static_in = torch.empty_like(images).requires_grad_(False)
@@ -223,7 +229,7 @@ class HalfStepGraphs:
             with torch.cuda.graph(graph, pool=self.pool, stream=self.stream):
                 outputs = body(static_in, step=(world == 1 and step))
                 if world > 1 and with_tail:
-                    self._tail(kind)
+                    self._tail(kind, static_in)
         finally:
             if gc_was_enabled:
                 gc.enable()

@@ -55,7 +55,7 @@ class MultiTensorAdam:
     @torch.no_grad()
     def step(self, grads=None, grad_scale=1.0, guard=None):
         """guard: a ``NonfiniteGuard`` — scan the gradients this update reads and drop the update on the device when any
-        element is not finite (opt.skip_nonfinite_steps)"""
+        element is not finite (opt.skip_nonfinite_steps).  Returns the guard's device skip word (None without a guard)."""
         st = self._state()
         g = self.param_groups[0]
         if grads is None:
@@ -69,6 +69,7 @@ class MultiTensorAdam:
         kw = {} if guard is None else {"skip": guard.scan(grads, st.sizes_t, self._cache)}
         backend.kernels().adam_step(params, grads, st.offsets_t, st.sizes_t, st.exp_avg, st.exp_avg_sq, st.steps, g["lr"],
                                     g["betas"][0], g["betas"][1], g["eps"], float(grad_scale), self._cache, **kw)
+        return kw.get("skip")
 
     # torch.optim.Adam's on-disk format, so optimizer checkpoints interoperate with the stock optimizer
     def state_dict(self):
@@ -123,6 +124,48 @@ class NonfiniteGuard:
         return total
 
 
+class ParameterEMA:
+    """Exponential moving average of one parameter group (opt.ema_kimg; INTEGRATION.md §2f): a flat shadow in the layout of
+    the group's ``MultiTensorAdam`` moments, initialised to a copy of the parameters, and the number of averaging updates
+    made, both on the device.  ``update`` is one launch pair (sae_ema_update) that forms beta from that counter on the
+    device, so it is capturable and one captured graph serves every step of the ramp."""
+
+    def __init__(self, adam, names, half_life_images, rampup):
+        self.adam = adam                      # layout (offsets_t, sizes_t) and pointer-table cache
+        self.names = list(names)              # state_dict keys of adam.params
+        self.half_life_images = float(half_life_images)
+        self.rampup = float(rampup)
+        adam._state()
+        p0 = adam.params[0]
+        self.shadow = torch.zeros(adam._total, dtype=p0.dtype, device=p0.device)
+        self.updates = torch.zeros(1, dtype=torch.int64, device=p0.device)
+        with torch.no_grad():
+            for v, p in zip(self.averaged(), adam.params):
+                v.copy_(p)
+
+    def averaged(self):
+        """one view of the shadow per parameter, shaped like it"""
+        return [self.shadow[o:o + n].view_as(p) for o, n, p in zip(self.adam._offsets, self.adam._sizes, self.adam.params)]
+
+    @torch.no_grad()
+    def update(self, images_per_update, skip=None):
+        """one averaging update after the group's Adam update; images_per_update: the update's global batch (rank's images
+        times world); skip: the guard's device skip word of that Adam update (a dropped update drops this one too)"""
+        st = self.adam._state()
+        backend.kernels().ema_update(self.adam.params, st.offsets_t, st.sizes_t, self.shadow, self.updates,
+                                     float(images_per_update), self.half_life_images, self.rampup, st._cache, skip=skip)
+
+    def state_dict(self):
+        return {"shadow": {n: v.detach().clone() for n, v in zip(self.names, self.averaged())}, "t": int(self.updates.item())}
+
+    def load_state_dict(self, sd):
+        """in place: captured graphs hold the shadow and the counter"""
+        with torch.no_grad():
+            for n, v in zip(self.names, self.averaged()):
+                v.copy_(sd["shadow"][n])
+            self.updates.fill_(int(sd["t"]))
+
+
 NONFINITE_KINDS = ("D", "R1", "G")
 
 
@@ -137,6 +180,12 @@ class SwappingAutoencoderOptimizer:
         parser.add_argument("--micro_batches", default=1, type=int,
                             help="gradient accumulation (extension): split each rank's batch into this many micro-batches and "
                                  "make one Adam update from their summed gradients")
+        parser.add_argument("--ema_kimg", default=0.0, type=float,
+                            help="weight averaging (extension): half-life, in thousands of images, of an exponential moving "
+                                 "average of the E and G weights, saved as <N>k_ema_checkpoint.pth; 0 turns it off")
+        parser.add_argument("--ema_rampup", default=0.05, type=float,
+                            help="ramp-up of the average's half-life: at most this fraction of the images seen so far; "
+                                 "0: no ramp")
         return parser
 
     def __init__(self, model):
@@ -165,6 +214,32 @@ class SwappingAutoencoderOptimizer:
         # skip-on-non-finite guard (extension, ``opt.skip_nonfinite_steps``): created on first use
         self._nonfinite_skipped = None      # device int64 [3]: skipped half-steps per kind, NONFINITE_KINDS order
         self._nonfinite_guards = {}
+        # weight averaging (extension, ``opt.ema_kimg`` > 0): the shadow is a copy of E and G as they are now, after any
+        # continue_train checkpoint the model loaded
+        self.ema = None
+        ema_kimg, ema_rampup = float(getattr(opt, "ema_kimg", 0.0)), float(getattr(opt, "ema_rampup", 0.05))
+        if not (ema_kimg >= 0.0 and ema_rampup >= 0.0):
+            raise ValueError("opt.ema_kimg and opt.ema_rampup must be >= 0, got %r and %r" % (ema_kimg, ema_rampup))
+        if ema_kimg > 0.0:
+            names = {id(p): n for n, p in self._inner().named_parameters()}
+            self.ema = ParameterEMA(self.optimizer_G, [names[id(p)] for p in self.Gparams], ema_kimg * 1000.0, ema_rampup)
+
+    def _inner(self):
+        return getattr(self.model, "singlegpu_model", self.model)
+
+    def ema_key(self):
+        """what a captured G graph bakes in of the average: () when it is off, so the graph keys stay as they were"""
+        return () if self.ema is None else (("ema", self.ema.half_life_images, self.ema.rampup),)
+
+    def ema_state_dict(self):
+        """the inner model's full state_dict with every E. / G. parameter replaced by its average (copies): the reference's
+        keys, shapes and dtypes, D, Dpatch and num_discriminator_iters live.  ``model.load`` takes it as it is."""
+        if self.ema is None:
+            raise RuntimeError("no weight average: opt.ema_kimg is 0")
+        sd = self._inner().state_dict()
+        for n, v in zip(self.ema.names, self.ema.averaged()):
+            sd[n] = v.detach().clone()
+        return sd
 
     def nonfinite_guard_on(self):
         return bool(getattr(self.opt, "skip_nonfinite_steps", False))
@@ -203,20 +278,26 @@ class SwappingAutoencoderOptimizer:
         params = self.Gparams if kind == "G" else self.Dparams
         return {names[id(p)]: c for p, c in zip(params, g.report.tolist()) if c}
 
-    def exchange_and_step(self, optimizer, params, kind=None, micro_batches=1):
+    def exchange_and_step(self, optimizer, params, kind=None, micro_batches=1, images=None):
         """optimizer step of one half-step; with more than one rank: pack -> all-reduce (SUM) -> Adam reading the bucket.
         With ``opt.skip_nonfinite_steps`` the gradients Adam reads (the reduced bucket with more than one rank: the same bytes
         on every rank) are scanned first and a non-finite one drops the update of the half-step ``kind``.
         micro_batches > 1: the gradients were summed into the bucket by ``accumulate_to_bucket`` after every micro-batch; one
-        all-reduce (world > 1), one scan, one Adam update reading the bucket with grad_scale = 1 / (micro_batches * world)."""
+        all-reduce (world > 1), one scan, one Adam update reading the bucket with grad_scale = 1 / (micro_batches * world).
+        With ``opt.ema_kimg`` > 0 a G update is followed by one averaging update over ``images`` (this rank's images of the
+        update) times world, dropped with the Adam update when the guard drops that."""
         guard = self.nonfinite_guard(kind) if kind is not None and self.nonfinite_guard_on() else None
         kw = {} if guard is None else {"guard": guard}
         if micro_batches > 1:
-            optimizer.step(grads=self.model.reduce_accumulated(), grad_scale=1.0 / (micro_batches * self.world), **kw)
+            skip = optimizer.step(grads=self.model.reduce_accumulated(), grad_scale=1.0 / (micro_batches * self.world), **kw)
         elif self.world > 1:
-            optimizer.step(grads=self.model.reduce_to_bucket(params), grad_scale=1.0 / self.world, **kw)
+            skip = optimizer.step(grads=self.model.reduce_to_bucket(params), grad_scale=1.0 / self.world, **kw)
         else:
-            optimizer.step(**kw)
+            skip = optimizer.step(**kw)
+        if kind == "G" and self.ema is not None:
+            if images is None:
+                raise ValueError("exchange_and_step: a G update with weight averaging needs its image count")
+            self.ema.update(images * self.world, skip=skip)
 
     @staticmethod
     def set_requires_grad(params, requires_grad):
@@ -250,7 +331,7 @@ class SwappingAutoencoderOptimizer:
         g_losses, g_metrics = self.model(images, None, None, command="compute_generator_losses")
         sum(v.mean() for v in g_losses.values()).backward()
         if step:
-            self.exchange_and_step(self.optimizer_G, self.Gparams, kind="G")
+            self.exchange_and_step(self.optimizer_G, self.Gparams, kind="G", images=images.shape[0])
         g_losses.update(g_metrics)
         return g_losses
 
@@ -328,7 +409,8 @@ class SwappingAutoencoderOptimizer:
             with torch.no_grad():
                 parts.append({key: (v.detach().clone() if key in ("_sp", "_gl") else v.detach().mean())
                               for key, v in out.items() if torch.is_tensor(v)})
-        self.exchange_and_step(self.optimizer_G if kind == "G" else self.optimizer_D, params, kind=kind, micro_batches=k)
+        self.exchange_and_step(self.optimizer_G if kind == "G" else self.optimizer_D, params, kind=kind, micro_batches=k,
+                               images=images.shape[0])
         return self._mean_outputs(parts)
 
     def train_generator_one_step(self, images):
@@ -364,11 +446,14 @@ class SwappingAutoencoderOptimizer:
     def state_dict(self):
         """Adam state of both groups (torch.optim.Adam's format) + the schedule counters.  The reference never saves this
         (optimizers/base_optimizer.py has no state I/O): resuming there restarts Adam's moments from zero.  With
-        ``opt.skip_nonfinite_steps`` the guard's skip counters (``nonfinite_steps()``) are saved as well."""
+        ``opt.skip_nonfinite_steps`` the guard's skip counters (``nonfinite_steps()``) are saved as well, with ``opt.ema_kimg``
+        > 0 the weight average under "ema" (``ParameterEMA.state_dict``: the shadow by state_dict key, and t)."""
         sd = {"optimizer_G": self.optimizer_G.state_dict(), "optimizer_D": self.optimizer_D.state_dict(),
               "train_mode_counter": self.train_mode_counter, "discriminator_iter_counter": self.discriminator_iter_counter}
         if self.nonfinite_guard_on():
             sd["nonfinite_steps"] = self.nonfinite_steps()
+        if self.ema is not None:
+            sd["ema"] = self.ema.state_dict()
         return sd
 
     def load_state_dict(self, sd):
@@ -379,22 +464,30 @@ class SwappingAutoencoderOptimizer:
         if "nonfinite_steps" in sd:
             counts = [int(sd["nonfinite_steps"].get(k, 0)) for k in NONFINITE_KINDS]
             self._nonfinite_counters().copy_(torch.tensor(counts, dtype=torch.int64))     # in place: captured graphs hold it
+        if self.ema is not None and "ema" in sd:
+            self.ema.load_state_dict(sd["ema"])          # without one the construction-time copy stays
 
-    def _optimizer_path(self, total_steps_so_far=None):
-        inner = getattr(self.model, "singlegpu_model", self.model)
-        name = "latest_optimizer.pth" if total_steps_so_far is None else "%dk_optimizer.pth" % (total_steps_so_far // 1000)
-        return os.path.join(inner._checkpoint_dir(), name)
+    def _optimizer_path(self, total_steps_so_far=None, what="optimizer"):
+        name = "latest_%s.pth" % what if total_steps_so_far is None else "%dk_%s.pth" % (total_steps_so_far // 1000, what)
+        return os.path.join(self._inner()._checkpoint_dir(), name)
+
+    @staticmethod
+    def _save_with_link(obj, path, link):
+        torch.save(obj, path)
+        if os.path.lexists(link):
+            os.remove(link)
+        os.symlink(os.path.basename(path), link)
 
     def save(self, total_steps_so_far):
-        """model checkpoint in the reference's format (models/base_model.py:33-41) + ``<N>k_optimizer.pth`` beside it"""
+        """model checkpoint in the reference's format (models/base_model.py:33-41) + ``<N>k_optimizer.pth`` beside it; with
+        ``opt.ema_kimg`` > 0 also ``<N>k_ema_checkpoint.pth`` (``ema_state_dict()``, the model checkpoint's format, so the
+        reference's ``--resume_iter latest_ema`` loads it) and its ``latest_ema_checkpoint.pth`` link.  Rank 0 writes."""
         self.model.save(total_steps_so_far)
         if getattr(self.model, "rank", 0) == 0:
-            path = self._optimizer_path(total_steps_so_far)
-            torch.save(self.state_dict(), path)
-            link = self._optimizer_path(None)
-            if os.path.lexists(link):
-                os.remove(link)
-            os.symlink(os.path.basename(path), link)
+            self._save_with_link(self.state_dict(), self._optimizer_path(total_steps_so_far), self._optimizer_path(None))
+            if self.ema is not None:
+                self._save_with_link(self.ema_state_dict(), self._optimizer_path(total_steps_so_far, "ema_checkpoint"),
+                                     self._optimizer_path(None, "ema_checkpoint"))
 
     def load(self, path=None):
         """restore the optimizer state written by ``save`` (missing file: keep the fresh state, like the reference)"""

@@ -45,6 +45,11 @@ def default_options(**overrides):
         # and one Adam update is made from their summed gradients, so the global batch no longer has to fit one pass per GPU
         # (SwappingAutoencoderOptimizer.split_micro_batches; INTEGRATION.md §2e)
         micro_batches=1,
+        # extension: weight averaging — after every G update an exponential moving average of the E and G weights moves towards
+        # them, with this half-life in thousands of images (0: off) and StyleGAN2-ADA's ramp-up (the half-life is at most
+        # ema_rampup times the images seen so far; 0: no ramp); trainer.save writes it as <N>k_ema_checkpoint.pth
+        # (optimizer.ParameterEMA; INTEGRATION.md §2f)
+        ema_kimg=0.0, ema_rampup=0.05,
     )
     for k, v in overrides.items():
         setattr(opt, k, v)
