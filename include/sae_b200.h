@@ -31,7 +31,7 @@ extern "C" {
 #define SAE_E_UNSUPPORTED  -3   /* valid request this build has no kernel for                */
 
 /* ABI version of this header; bumped on any signature change. */
-#define SAE_ABI_VERSION 18
+#define SAE_ABI_VERSION 19
 int         sae_abi_version(void);
 const char* sae_last_error(void);
 /* number of kernels launched by this library in the calling process since load
@@ -354,6 +354,42 @@ int sae_adam_step_guarded(float* const* p_ptrs, const float* const* g_ptrs, cons
 int sae_ema_update(const float* const* p_ptrs, const int64_t* offsets, const int64_t* sizes, int n, float* shadow,
                    int64_t total, int64_t* updates, float batch_images, float half_life_images, float rampup,
                    const unsigned long long* skip, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Training statistics (ABI 19; SwappingAutoencoderOptimizer with opt.training_stats, INTEGRATION §2g).  fp64 sums ADDED into
+ * caller-owned accumulators, so a window accumulates over many updates until the caller reads and clears it.  No float
+ * atomics: every tensor is split over SAE_STATS_BLOCKS blocks by a partition that depends on its size alone (not on the
+ * alignment of the view), the blocks store partials into `partials`, and a second launch adds each tensor's partials in
+ * block order.  Results are bitwise reproducible; deterministic mode needs no twin.  64-bit indexing, any alignment (16-byte
+ * aligned data is read as float4).  Bad arguments: SAE_E_INVALID before any CUDA call.
+ * sae_sumsq: out[t] += scale^2 * sum_i x_t[i]^2 (fp64, scale widened from fp32) for every non-NULL ptrs[t], t < n.  ptrs /
+ *   sizes: device arrays of n pointers / int64 element counts, as for sae_nonfinite_count; partials: device workspace of
+ *   n * SAE_STATS_BLOCKS doubles; skip (may be NULL): when *skip != 0, read on the device, nothing is added.  n in [0, 65535],
+ *   scale finite.
+ * sae_adam_norms: after a sae_adam_step (or _guarded) with the same tables, moments, step counts and hyper-parameters:
+ *   weight_out[t] += sum_i p_t[i]^2 for every non-NULL p_ptrs[t], and update_out[t] += sum_i d_t[i]^2 with Adam's step
+ *   recomputed in its own fp32 expression  d = lr / (1 - beta1^s) * m / (sqrtf(v) / sqrtf(1 - beta2^s) + eps),  s = steps[t]
+ *   (already advanced), m / v the updated moments at offsets[t]; a tensor with g_ptrs[t] == NULL (skipped by Adam) adds 0
+ *   to update_out.  updates (may be NULL): *updates += 1.  skip (may be NULL): when *skip != 0 nothing is added, *updates
+ *   included, so a dropped update leaves every accumulator bitwise unchanged.  partials: 2 * n * SAE_STATS_BLOCKS doubles.
+ * sae_score_stats: acc[0] += sum of the finite elements of x, acc[1] += sum of their signs (+1, -1, 0 for +-0), acc[2] +=
+ *   number of finite elements, acc[3] += number of NaN / +-Inf elements.  x: fp32 device tensor of ndim in [1, 4] dimensions
+ *   (host arrays sizes / strides, in elements, outermost first, strides >= 0); acc: 4 device doubles.  One block: meant for
+ *   the small logit tensors of the discriminators.  An empty tensor launches nothing.
+ * C caller, one G update of n tensors with the window buffers grad_sq[n], weight_sq[n], step_sq[n], count[1]:
+ *   sae_nonfinite_count(g_tab, sizes, n, counts, s);                                  optional guard, as in §2d
+ *   sae_adam_step_guarded(p_tab, g_tab, offsets, sizes, n, m, v, steps, lr, b1, b2, eps, gs, counts + n, s);
+ *   sae_sumsq(g_tab, sizes, n, gs, grad_sq, ws, counts + n, s);
+ *   sae_adam_norms(p_tab, g_tab, offsets, sizes, n, m, v, steps, lr, b1, b2, eps, weight_sq, step_sq, count, ws, counts + n, s);
+ * ------------------------------------------------------------------------------------------ */
+#define SAE_STATS_BLOCKS 128
+int sae_sumsq(const float* const* ptrs, const int64_t* sizes, int n, float scale, double* out, double* partials,
+              const unsigned long long* skip, void* stream);
+int sae_adam_norms(const float* const* p_ptrs, const float* const* g_ptrs, const int64_t* offsets, const int64_t* sizes, int n,
+                   const float* exp_avg, const float* exp_avg_sq, const float* steps, float lr, float beta1, float beta2,
+                   float eps, double* weight_out, double* update_out, double* updates, double* partials,
+                   const unsigned long long* skip, void* stream);
+int sae_score_stats(const float* x, int ndim, const int64_t* sizes, const int64_t* strides, double* acc, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Random-crop resampler of the patch discriminator (SURVEY.md §8 f1).  Replaces

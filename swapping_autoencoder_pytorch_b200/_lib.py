@@ -12,7 +12,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsae_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
 
-SAE_ABI_VERSION = 18
+SAE_ABI_VERSION = 19
+SAE_STATS_BLOCKS = 128          # header: partials workspace rows of sae_sumsq / sae_adam_norms
 SAE_E_UNSUPPORTED = -3        # a valid request no kernel of this build takes (header: SAE_E_*)
 
 c_float_p = ctypes.c_void_p   # raw device pointers travel as integers
@@ -120,6 +121,11 @@ SIGNATURES = {
     "sae_nonfinite_count": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, c_stream]),
     "sae_ema_update": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, c_float_p, ctypes.c_int64,
                                       ctypes.c_void_p] + [ctypes.c_float] * 3 + [ctypes.c_void_p, c_stream]),
+    "sae_sumsq": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p,
+                                 ctypes.c_void_p, c_stream]),
+    "sae_adam_norms": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int] + [c_float_p] * 3 + [ctypes.c_float] * 4
+                       + [ctypes.c_void_p] * 5 + [c_stream]),
+    "sae_score_stats": (ctypes.c_int, [c_float_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, c_stream]),
     "sae_crop_gather": (ctypes.c_int, [c_float_p] * 5 + [ctypes.c_int] * 7 + [ctypes.c_int64] * 4 + [ctypes.c_int, c_stream]),
     "sae_crop_gather_backward": (ctypes.c_int, [c_float_p] * 5 + [ctypes.c_int] * 6 + [ctypes.c_int64] * 4 + [c_stream]),
     "sae_torgb_forward": (ctypes.c_int, [c_float_p] * 5 + [ctypes.c_int] * 4 + [ctypes.c_float, ctypes.c_int, c_stream]),

@@ -90,6 +90,13 @@ def _need_int64(t):
         raise _lib.SaeError("non-finite guard counters must be contiguous int64 CUDA tensors")
 
 
+def _need_fp64(*ts):
+    """the fp64 accumulators of the training statistics (None: an optional argument left out)"""
+    for t in ts:
+        if t is not None and (not t.is_cuda or t.dtype != torch.float64 or not t.is_contiguous()):
+            raise _lib.SaeError("training-statistics accumulators must be contiguous fp64 CUDA tensors")
+
+
 class PointerTables:
     """Device copies of host address lists (tuples of ``data_ptr()``), cached by content.  The pinned staging rows are
     allocated up front — a miss costs a device allocation and an async copy, so a miss inside a CUDA-graph capture is legal:
@@ -570,6 +577,54 @@ class CudaKernels:
         p_tab = cache.get(tuple(p.data_ptr() for p in params))
         self._launch(shadow.device, "sae_ema_update", _ptr(p_tab), _ptr(offsets), _ptr(sizes), len(params), _ptr(shadow),
                      shadow.numel(), _ptr(updates), float(batch_images), float(half_life_images), float(rampup), _ptr(skip))
+
+    # ----------------------------------------------------------------- training statistics (INTEGRATION §2g)
+    def sumsq(self, tensors, sizes, out, partials, cache, scale=1.0, skip=None):
+        """out[i] += scale^2 * sum of squares of tensors[i] (None: skipped), in fp64 (sae_sumsq).  tensors: contiguous fp32 CUDA
+        tensors; sizes: device int64 tensor of their element counts; out: device fp64 tensor of n entries; partials: device
+        fp64 workspace of at least n * _lib.SAE_STATS_BLOCKS entries; cache: ``PointerTables``.  skip: optional one-element
+        device int64 tensor; a non-zero value adds nothing."""
+        for t in tensors:
+            _need_cuda(t)
+        _need_fp64(out, partials)
+        if skip is not None:
+            _need_int64(skip)
+        if out.numel() < len(tensors) or partials.numel() < len(tensors) * _lib.SAE_STATS_BLOCKS:
+            raise _lib.SaeError("sumsq: out needs n entries and partials n * SAE_STATS_BLOCKS")
+        tab = cache.get(tuple(0 if t is None else t.data_ptr() for t in tensors))
+        self._launch(out.device, "sae_sumsq", _ptr(tab), _ptr(sizes), len(tensors), float(scale), _ptr(out), _ptr(partials),
+                     _ptr(skip))
+
+    def adam_norms(self, params, grads, offsets, sizes, exp_avg, exp_avg_sq, steps, lr, beta1, beta2, eps, weight_out,
+                   update_out, updates, partials, cache, skip=None):
+        """After ``adam_step`` with the same arguments: weight_out[i] += |params[i]|^2 and update_out[i] += |Adam's step|^2
+        (0 where grads[i] is None), the step recomputed from the moments and step counts; updates += 1 (sae_adam_norms).
+        weight_out / update_out: device fp64 tensors of n entries; updates: one-element device fp64 tensor or None; partials:
+        device fp64 workspace of at least 2 * n * _lib.SAE_STATS_BLOCKS entries.  skip: as for ``adam_step``; a non-zero value
+        adds nothing, to the counter included."""
+        _need_cuda(exp_avg, exp_avg_sq, steps, *params)
+        _need_fp64(weight_out, update_out, updates, partials)
+        if skip is not None:
+            _need_int64(skip)
+        n = len(params)
+        if weight_out.numel() < n or update_out.numel() < n or partials.numel() < 2 * n * _lib.SAE_STATS_BLOCKS:
+            raise _lib.SaeError("adam_norms: outputs need n entries and partials 2 * n * SAE_STATS_BLOCKS")
+        p_tab = cache.get(tuple(p.data_ptr() for p in params))
+        g_tab = cache.get(tuple(0 if g is None else g.data_ptr() for g in grads))
+        self._launch(exp_avg.device, "sae_adam_norms", _ptr(p_tab), _ptr(g_tab), _ptr(offsets), _ptr(sizes), n, _ptr(exp_avg),
+                     _ptr(exp_avg_sq), _ptr(steps), float(lr), float(beta1), float(beta2), float(eps), _ptr(weight_out),
+                     _ptr(update_out), _ptr(updates), _ptr(partials), _ptr(skip))
+
+    def score_stats(self, x, acc):
+        """acc[0:4] += (sum, sum of signs, count) of the finite elements of x and the count of its NaN / +-Inf elements
+        (sae_score_stats).  x: fp32 CUDA tensor of 1 to 4 dimensions, any non-negative strides; acc: device fp64 tensor."""
+        _need_cuda(x, strided=True)
+        _need_fp64(acc)
+        if acc.numel() < 4 or not 1 <= x.dim() <= 4:
+            raise _lib.SaeError("score_stats: needs a 1- to 4-dimensional tensor and 4 accumulators")
+        shape = (ctypes.c_int64 * x.dim())(*x.shape)
+        strides = (ctypes.c_int64 * x.dim())(*x.stride())
+        self._launch(acc.device, "sae_score_stats", _ptr(x), x.dim(), shape, strides, _ptr(acc))
 
     # ----------------------------------------------------------------- ToRGB
     def torgb_forward(self, x, s, w, bias, wscale):

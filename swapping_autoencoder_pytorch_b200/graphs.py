@@ -19,6 +19,8 @@ images copied into a static input buffer.
 * Weight averaging (opt.ema_kimg > 0): the averaging update follows the G update's Adam wherever that runs (inside the G
   graph at world size 1); it forms beta on the device from a counter that lives outside the pool, so one graph serves every
   step of the ramp.
+* Training statistics (opt.training_stats): the score launches sit in the model's forward and the norm launches follow
+  the Adam update wherever that runs; both add into a window that lives outside the pool.
 * A body that fails to capture falls back to eager execution for the rest of the run (``self.disabled`` holds why).
 """
 import gc
@@ -37,7 +39,8 @@ class HalfStepGraphs:
         self.warmup = warmup
         self.calls = {}
         # (kind, input shape, kernel precision, deterministic, non-finite guard[, micro-batches when > 1][, the average's
-        # setting for G when it is on]) -> (graph, static_input, static_outputs, launches, ...)
+        # setting for G when it is on][, ("stats",) when the statistics are on]) -> (graph, static_input, static_outputs,
+        # launches, ...)
         self.captured = {}
         self.pool = None
         self.stream = None             # side stream shared by the eager warm-up calls and every capture (see _side)
@@ -111,7 +114,8 @@ class HalfStepGraphs:
         # graphs, after warm-up calls of their own (the other mode's kernels initialise lazily, outside any capture).  The same
         # holds for the deterministic mode (backend.CudaKernels.deterministic_mode()), which records other kernels, and for the
         # non-finite guard (opt.skip_nonfinite_steps), which adds the scan and the guarded update, and for the weight average
-        # (opt.ema_kimg), whose launch the G graph holds.
+        # (opt.ema_kimg), whose launch the G graph holds, and for the training statistics (opt.training_stats), whose launches
+        # every graph holds.
         k = backend.kernels()
         precision = getattr(k, "precision", "tf32")
         det = bool(getattr(k, "deterministic_mode", lambda: False)())
@@ -119,6 +123,7 @@ class HalfStepGraphs:
         extra = () if step else (micro_batches,)          # k = 1 keeps the keys it always had
         if kind == "G":
             extra += self.trainer.ema_key()                # () with the average off
+        extra += self.trainer.stats_key()                  # () with the statistics off
         n = self.calls.get((kind, precision, det, guard) + extra, 0)
         self.calls[(kind, precision, det, guard) + extra] = n + 1
         key = (kind, tuple(images.shape), precision, det, guard) + extra

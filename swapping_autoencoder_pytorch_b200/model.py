@@ -109,6 +109,11 @@ class BaseModel(torch.nn.Module):
 
 
 class SwappingAutoencoderModel(BaseModel):
+    # training statistics (extension, opt.training_stats): the trainer sets this to a callable ``sink(kind, name, logits)``
+    # that is handed every discriminator logit tensor of the D ("D") and G ("G") losses, R1 aside (optimizer.TrainingStats).
+    # It only reads them: losses and random draws are the same with and without it.
+    score_sink = None
+
     @staticmethod
     def modify_commandline_options(parser, is_train):
         BaseModel.modify_commandline_options(parser, is_train)
@@ -164,6 +169,9 @@ class SwappingAutoencoderModel(BaseModel):
             pred_real, pred_rec, pred_mix = self.D(torch.cat([real, rec, mix])).split([real.size(0), rec.size(0), mix.size(0)])
         else:
             pred_real, pred_rec, pred_mix = self.D(real), self.D(rec), self.D(mix)
+        if self.score_sink is not None:
+            for name, pred in (("real", pred_real), ("rec", pred_rec), ("mix", pred_mix)):
+                self.score_sink("D", name, pred)
         return {
             "D_real": util.gan_loss(pred_real, should_be_classified_as_real=True) * lam,
             "D_rec": util.gan_loss(pred_rec, should_be_classified_as_real=False) * (0.5 * lam),
@@ -188,11 +196,14 @@ class SwappingAutoencoderModel(BaseModel):
             real_feat = self.Dpatch.extract_features(self.get_random_crops(real), aggregate=opt.patch_use_aggregation)
             target_feat = self.Dpatch.extract_features(self.get_random_crops(real))
             mix_feat = self.Dpatch.extract_features(self.get_random_crops(mix))
+        pred_real = self.Dpatch.discriminate_features(real_feat, target_feat)
+        pred_mix = self.Dpatch.discriminate_features(real_feat, mix_feat)
+        if self.score_sink is not None:
+            self.score_sink("D", "patch_real", pred_real)
+            self.score_sink("D", "patch_mix", pred_mix)
         return {
-            "PatchD_real": util.gan_loss(self.Dpatch.discriminate_features(real_feat, target_feat),
-                                         should_be_classified_as_real=True) * opt.lambda_PatchGAN,
-            "PatchD_mix": util.gan_loss(self.Dpatch.discriminate_features(real_feat, mix_feat),
-                                        should_be_classified_as_real=False) * opt.lambda_PatchGAN,
+            "PatchD_real": util.gan_loss(pred_real, should_be_classified_as_real=True) * opt.lambda_PatchGAN,
+            "PatchD_mix": util.gan_loss(pred_mix, should_be_classified_as_real=False) * opt.lambda_PatchGAN,
         }
 
     def compute_discriminator_losses(self, real):
@@ -256,14 +267,19 @@ class SwappingAutoencoderModel(BaseModel):
                 pred_rec, pred_mix = self.D(torch.cat([rec, mix])).split([rec.size(0), mix.size(0)])
             else:
                 pred_rec, pred_mix = self.D(rec), self.D(mix)
+            if self.score_sink is not None:
+                self.score_sink("G", "rec", pred_rec)
+                self.score_sink("G", "mix", pred_mix)
             losses["G_GAN_rec"] = util.gan_loss(pred_rec, should_be_classified_as_real=True) * (opt.lambda_GAN * 0.5)
             losses["G_GAN_mix"] = util.gan_loss(pred_mix, should_be_classified_as_real=True) * (opt.lambda_GAN * 1.0)
         if opt.lambda_PatchGAN > 0.0:
             real_feat = self.Dpatch.extract_features(self.get_random_crops(real),
                                                      aggregate=opt.patch_use_aggregation).detach()
             mix_feat = self.Dpatch.extract_features(self.get_random_crops(mix))
-            losses["G_mix"] = util.gan_loss(self.Dpatch.discriminate_features(real_feat, mix_feat),
-                                            should_be_classified_as_real=True) * opt.lambda_PatchGAN
+            pred_mix = self.Dpatch.discriminate_features(real_feat, mix_feat)
+            if self.score_sink is not None:
+                self.score_sink("G", "patch_mix", pred_mix)
+            losses["G_mix"] = util.gan_loss(pred_mix, should_be_classified_as_real=True) * opt.lambda_PatchGAN
         return losses, metrics
 
     # ------------------------------------------------------------------ inference callers (SURVEY.md §8 f4)

@@ -5,11 +5,12 @@ hyper-parameters and R1 schedule) for boxes without the reference checkout.  The
 exchange is invisible here: ``MultiGPUModelWrapper`` (parallel.py) all-reduces the active parameter group at
 the end of every ``backward()``.
 """
+import math
 import os
 
 import torch
 
-from . import backend, util
+from . import _lib, backend, util
 
 
 class MultiTensorAdam:
@@ -169,6 +170,95 @@ class ParameterEMA:
 NONFINITE_KINDS = ("D", "R1", "G")
 
 
+# the discriminator logits the model hands to the statistics' sink (model.SwappingAutoencoderModel.score_sink), by half-step
+STATS_SCORES = (("D", "real"), ("D", "rec"), ("D", "mix"), ("D", "patch_real"), ("D", "patch_mix"),
+                ("G", "rec"), ("G", "mix"), ("G", "patch_mix"))
+STATS_NORMS = ("grad_norm", "weight_norm", "update_norm")
+
+
+class TrainingStats:
+    """Training statistics accumulated on the device (opt.training_stats; INTEGRATION.md §2g).  One flat fp64 window holds,
+    per kind of update (D, R1, G): the number of applied updates, then per tensor the squared L2 norms of the gradient Adam
+    read (grad_scale included), of the parameter after the update and of the step Adam applied; after them four sums (score,
+    sign, finite count, non-finite count) per discriminator logit tensor of ``STATS_SCORES``.  ``record_update`` is four
+    launches (sae_sumsq, sae_adam_norms) after the group's Adam update and ``score`` one (sae_score_stats); none reads
+    anything back, so both are capturable.  ``read`` is the only device-to-host transfer."""
+
+    def __init__(self, groups, device, world=1):
+        self.groups = groups                    # {kind: (MultiTensorAdam, state_dict keys of its params)}
+        self.world = world
+        self._at, o = {}, 0
+        for kind in NONFINITE_KINDS:
+            self._at[kind] = o                  # [updates, grad_sq[n], weight_sq[n], update_sq[n]]
+            o += 1 + 3 * len(groups[kind][1])
+        self._scores_at = o
+        self.window = torch.zeros(o + 4 * len(STATS_SCORES), dtype=torch.float64, device=device)
+        n = max(len(names) for _, names in groups.values())
+        self.partials = torch.zeros(max(2 * n * _lib.SAE_STATS_BLOCKS, 1), dtype=torch.float64, device=device)
+        self._score_index = {k: i for i, k in enumerate(STATS_SCORES)}
+
+    def _views(self, kind):
+        o, n = self._at[kind], len(self.groups[kind][1])
+        w = self.window
+        return w[o:o + 1], w[o + 1:o + 1 + n], w[o + 1 + n:o + 1 + 2 * n], w[o + 1 + 2 * n:o + 1 + 3 * n]
+
+    @torch.no_grad()
+    def record_update(self, kind, grads, grad_scale, skip=None):
+        """after the Adam update of ``kind``: grads as that update read them (None: the parameters' .grad), grad_scale its
+        factor, skip the guard's device skip word (a dropped update adds nothing, to the update count included)"""
+        adam = self.groups[kind][0]
+        if grads is None:
+            grads = [p.grad for p in adam.params]
+        grads = [None if t is None else (t if t.is_contiguous() else t.contiguous()) for t in grads]
+        if all(t is None for t in grads):
+            return                              # MultiTensorAdam.step made no update either
+        st = adam._state()
+        g = adam.param_groups[0]
+        updates, grad_sq, weight_sq, update_sq = self._views(kind)
+        k = backend.kernels()
+        k.sumsq(grads, st.sizes_t, grad_sq, self.partials, st._cache, scale=float(grad_scale), skip=skip)
+        k.adam_norms(adam.params, grads, st.offsets_t, st.sizes_t, st.exp_avg, st.exp_avg_sq, st.steps, g["lr"], g["betas"][0],
+                     g["betas"][1], g["eps"], weight_sq, update_sq, updates, self.partials, st._cache, skip=skip)
+
+    @torch.no_grad()
+    def score(self, kind, name, logits):
+        """the model's sink: add one discriminator logit tensor of the ``kind`` half-step to the window"""
+        o = self._scores_at + 4 * self._score_index[(kind, name)]
+        backend.kernels().score_stats(logits.detach(), self.window[o:o + 4])
+
+    def read(self, reset=True, per_tensor=False):
+        """the window as plain floats (see SwappingAutoencoderOptimizer.training_stats); one device-to-host copy.  With more
+        than one rank the score sums are all-reduced first, so every rank must call this."""
+        src = self.window
+        if self.world > 1:
+            import torch.distributed as dist
+            scores = self.window[self._scores_at:].clone()
+            dist.all_reduce(scores)
+            src = torch.cat([self.window[:self._scores_at], scores])
+        vals = src.cpu().tolist()
+        if reset:
+            self.window.zero_()                 # in place: captured graphs hold the window
+        out, pt = {}, {}
+        for kind in NONFINITE_KINDS:
+            o, names = self._at[kind], self.groups[kind][1]
+            n, u = len(names), vals[self._at[kind]]
+            out[kind + "/updates"] = int(u)
+            for j, stat in enumerate(STATS_NORMS):
+                seg = vals[o + 1 + j * n:o + 1 + (j + 1) * n]
+                out["%s/%s" % (kind, stat)] = math.sqrt(sum(seg) / u) if u else 0.0
+                if per_tensor:
+                    for key, v in zip(names, seg):
+                        pt.setdefault(key, {})["%s/%s" % (kind, stat)] = math.sqrt(v / u) if u else 0.0
+        for i, (kind, name) in enumerate(STATS_SCORES):
+            s, sign, finite, bad = vals[self._scores_at + 4 * i:self._scores_at + 4 * i + 4]
+            out["%s/scores/%s" % (kind, name)] = s / finite if finite else 0.0
+            out["%s/signs/%s" % (kind, name)] = sign / finite if finite else 0.0
+            out["%s/scores/%s/nonfinite" % (kind, name)] = int(bad)
+        if per_tensor:
+            out["per_tensor"] = pt
+        return out
+
+
 class SwappingAutoencoderOptimizer:
     @staticmethod
     def modify_commandline_options(parser, is_train):
@@ -186,6 +276,9 @@ class SwappingAutoencoderOptimizer:
         parser.add_argument("--ema_rampup", default=0.05, type=float,
                             help="ramp-up of the average's half-life: at most this fraction of the images seen so far; "
                                  "0: no ramp")
+        parser.add_argument("--training_stats", type=util.str2bool, nargs="?", const=True, default=False,
+                            help="training statistics (extension): accumulate per-update gradient, weight and Adam-step norms "
+                                 "and the discriminators' scores on the device; read them with trainer.training_stats()")
         return parser
 
     def __init__(self, model):
@@ -223,6 +316,16 @@ class SwappingAutoencoderOptimizer:
         if ema_kimg > 0.0:
             names = {id(p): n for n, p in self._inner().named_parameters()}
             self.ema = ParameterEMA(self.optimizer_G, [names[id(p)] for p in self.Gparams], ema_kimg * 1000.0, ema_rampup)
+        # training statistics (extension, ``opt.training_stats``): the window lives outside any graph pool, like the shadow
+        self.stats = None
+        if getattr(opt, "training_stats", False) and self.Gparams:
+            names = {id(p): n for n, p in self._inner().named_parameters()}
+            d_names, g_names = [names[id(p)] for p in self.Dparams], [names[id(p)] for p in self.Gparams]
+            self.stats = TrainingStats({"D": (self.optimizer_D, d_names), "R1": (self.optimizer_D, d_names),
+                                        "G": (self.optimizer_G, g_names)}, self.Gparams[0].device, world=self.world)
+            inner = self._inner()
+            if hasattr(inner, "score_sink"):    # this package's model; the reference's own model file has no sink
+                inner.score_sink = self.stats.score
 
     def _inner(self):
         return getattr(self.model, "singlegpu_model", self.model)
@@ -230,6 +333,26 @@ class SwappingAutoencoderOptimizer:
     def ema_key(self):
         """what a captured G graph bakes in of the average: () when it is off, so the graph keys stay as they were"""
         return () if self.ema is None else (("ema", self.ema.half_life_images, self.ema.rampup),)
+
+    def stats_key(self):
+        """what a captured graph bakes in of the statistics: () when they are off, so the graph keys stay as they were"""
+        return () if self.stats is None else (("stats",),)
+
+    def training_stats(self, reset=True, per_tensor=False):
+        """The statistics accumulated since the last reset (opt.training_stats; INTEGRATION.md §2g), as plain floats, with
+        one device-to-host copy:
+        * "<kind>/updates" for kind in D, R1, G: the applied updates (a dropped one is in ``nonfinite_steps()`` instead);
+        * "<kind>/grad_norm", "/weight_norm", "/update_norm": the group's L2 norm of the gradient Adam read, of the parameters
+          after the update and of the step Adam applied, root-mean-square over the window's updates (0.0 without updates);
+        * "D/scores/<t>" and "D/signs/<t>" for t in real, rec, mix, patch_real, patch_mix, and "G/..." for rec, mix and
+          patch_mix: the mean discriminator logit and mean sign over the finite elements, "…/scores/<t>/nonfinite" the
+          number of NaN / Inf logits left out (these need this package's model: the reference's model file has no sink);
+        * per_tensor=True: "per_tensor", {state_dict key: {"<kind>/<norm>": float}}.
+        reset: clear the window afterwards.  With more than one rank this is a collective (one small all-reduce of the score
+        sums): every rank must call it.  The norms are the same on every rank already."""
+        if self.stats is None:
+            raise RuntimeError("no training statistics: opt.training_stats is off")
+        return self.stats.read(reset=reset, per_tensor=per_tensor)
 
     def ema_state_dict(self):
         """the inner model's full state_dict with every E. / G. parameter replaced by its average (copies): the reference's
@@ -285,15 +408,19 @@ class SwappingAutoencoderOptimizer:
         micro_batches > 1: the gradients were summed into the bucket by ``accumulate_to_bucket`` after every micro-batch; one
         all-reduce (world > 1), one scan, one Adam update reading the bucket with grad_scale = 1 / (micro_batches * world).
         With ``opt.ema_kimg`` > 0 a G update is followed by one averaging update over ``images`` (this rank's images of the
-        update) times world, dropped with the Adam update when the guard drops that."""
+        update) times world, dropped with the Adam update when the guard drops that.  With ``opt.training_stats`` the norms of
+        the update are added to the statistics' window, from the gradients Adam read; a dropped update adds nothing."""
         guard = self.nonfinite_guard(kind) if kind is not None and self.nonfinite_guard_on() else None
         kw = {} if guard is None else {"guard": guard}
         if micro_batches > 1:
-            skip = optimizer.step(grads=self.model.reduce_accumulated(), grad_scale=1.0 / (micro_batches * self.world), **kw)
+            grads, scale = self.model.reduce_accumulated(), 1.0 / (micro_batches * self.world)
         elif self.world > 1:
-            skip = optimizer.step(grads=self.model.reduce_to_bucket(params), grad_scale=1.0 / self.world, **kw)
+            grads, scale = self.model.reduce_to_bucket(params), 1.0 / self.world
         else:
-            skip = optimizer.step(**kw)
+            grads, scale = None, 1.0                # Adam reads the parameters' .grad
+        skip = optimizer.step(grads=grads, grad_scale=scale, **kw)
+        if self.stats is not None and kind is not None:
+            self.stats.record_update(kind, grads, scale, skip=skip)
         if kind == "G" and self.ema is not None:
             if images is None:
                 raise ValueError("exchange_and_step: a G update with weight averaging needs its image count")

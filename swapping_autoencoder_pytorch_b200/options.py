@@ -50,6 +50,10 @@ def default_options(**overrides):
         # ema_rampup times the images seen so far; 0: no ramp); trainer.save writes it as <N>k_ema_checkpoint.pth
         # (optimizer.ParameterEMA; INTEGRATION.md §2f)
         ema_kimg=0.0, ema_rampup=0.05,
+        # extension: training statistics — per-update gradient, weight and Adam-step norms of every group and the mean score and
+        # sign of every discriminator logit tensor, accumulated on the device until trainer.training_stats() reads them
+        # (optimizer.TrainingStats; INTEGRATION.md §2g)
+        training_stats=False,
     )
     for k, v in overrides.items():
         setattr(opt, k, v)
