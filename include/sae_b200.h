@@ -31,7 +31,7 @@ extern "C" {
 #define SAE_E_UNSUPPORTED  -3   /* valid request this build has no kernel for                */
 
 /* ABI version of this header; bumped on any signature change. */
-#define SAE_ABI_VERSION 19
+#define SAE_ABI_VERSION 20
 int         sae_abi_version(void);
 const char* sae_last_error(void);
 /* number of kernels launched by this library in the calling process since load
@@ -390,6 +390,48 @@ int sae_adam_norms(const float* const* p_ptrs, const float* const* g_ptrs, const
                    float eps, double* weight_out, double* update_out, double* updates, double* partials,
                    const unsigned long long* skip, void* stream);
 int sae_score_stats(const float* x, int ndim, const int64_t* sizes, const int64_t* strides, double* acc, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Adaptive discriminator augmentation (ABI 20; SwappingAutoencoderOptimizer with opt.augment_p > 0 or opt.ada_target > 0,
+ * INTEGRATION §2h): StyleGAN2-ADA's geometric and colour transforms of the images D sees.  Images are RGB (C = 3), fp32,
+ * never rounded to TF32.  No float atomics: every output element is written by one thread, so deterministic mode needs no
+ * twin.  Bad arguments: SAE_E_INVALID before any CUDA call; N == 0 launches nothing.
+ * A per-image record holds SAE_AUG_RECORD floats: [0, 9) G_inv (3x3, row-major; maps centred output to centred input pixel
+ * coordinates), [9, 25) C (4x4, row-major; rgb <- C[:3, :3] rgb + C[:3, 3]), the rest zero.
+ * sae_augment_params: rec[n] from u [N, SAE_AUG_UNIFORMS] ~ U[0, 1), z [N, SAE_AUG_NORMALS] ~ N(0, 1) and the device
+ *   scalar *p (fp32); gates u < p (the two free rotations u < 1 - sqrt(1 - p)); H, W: the image size (translations are
+ *   fractions of it).  The column layout is documented at aug_params_kernel (csrc/augment.cu).
+ * sae_augment_sample: s [N, 2(H + 6), 2(W + 6), 4] (contiguous, 16-byte aligned; channel 3 zero) = bilinear samples (zeros outside) on the G_inv-transformed
+ *   grid of U = upfirdn2d(reflect_pad(x, (W - 1, H - 1)), 4 * sym6 (x) sym6 / 2, up = 2, pad = (6, 5)); U is computed on the
+ *   fly.  x: logical [N, 3, H, W] addressed through element strides.  copy_identity: an image whose G_inv is exactly I is
+ *   written as zeros (sae_augment_color takes it from x).  H, W >= 2.
+ * sae_augment_sample_adjoint: dx [N, H, W, 3] (contiguous) = the adjoint of sae_augment_sample applied to ds (contiguous
+ *   [N, 2(H + 6), 2(W + 6), 4], channel 3 ignored); with copy_identity an image whose G_inv is exactly I copies channels
+ *   0..2 of gc [N, H, W, 4] instead.  ds and gc 16-byte aligned.
+ * sae_augment_color: out [N, H, W, 3] (contiguous) = C[:3, :3] v + offset * C[:3, 3], v = a[n, :, y, x] (strided, logical
+ *   NCHW) for an image whose G_inv is exactly I when copy_identity is set, else channels 0..2 of b [N, H, W, 4] (contiguous,
+ *   16-byte aligned); a C that is exactly I copies v.
+ * sae_augment_color_adjoint: gc [N, H, W, 4] (contiguous, 16-byte aligned; channel 3 zero) = C[:3, :3]^T dy[n, :, y, x]
+ *   (strided, logical NCHW).  The 4-channel intermediates let the FIR kernels read one float4 per pixel.
+ *   The full operator is  color(x, upfirdn2d(sample(x), sym6 (x) sym6 / 2 flipped, down = 2, pad = (-1, -1))), and its
+ *   adjoint  sample_adjoint(upfirdn2d-adjoint(gc), gc)  with gc = color_adjoint(dy).
+ * sae_ada_adjust: one thread.  acc: the 4 doubles of sae_score_stats over D(real).  If acc[2] > 0:
+ *   *p = max(0, *p + (float)(sign(acc[1] / acc[2] - target) * step)), the sign and product in fp64; then acc[0..3] = 0.
+ *   step finite and >= 0, target finite.
+ * ------------------------------------------------------------------------------------------ */
+#define SAE_AUG_UNIFORMS 21
+#define SAE_AUG_NORMALS 7
+#define SAE_AUG_RECORD 32
+int sae_augment_params(const float* u, const float* z, const float* p, float* rec, int N, int H, int W, void* stream);
+int sae_augment_sample(const float* x, const float* rec, float* s, int N, int H, int W, int64_t xs_n, int64_t xs_c,
+                       int64_t xs_h, int64_t xs_w, int copy_identity, void* stream);
+int sae_augment_sample_adjoint(const float* ds, const float* gc, const float* rec, float* dx, int N, int H, int W,
+                               int copy_identity, void* stream);
+int sae_augment_color(const float* a, const float* b, const float* rec, float* out, int N, int H, int W, int64_t as_n,
+                      int64_t as_c, int64_t as_h, int64_t as_w, int offset, int copy_identity, void* stream);
+int sae_augment_color_adjoint(const float* dy, const float* rec, float* gc, int N, int H, int W, int64_t ds_n, int64_t ds_c,
+                              int64_t ds_h, int64_t ds_w, void* stream);
+int sae_ada_adjust(float* p, double* acc, double step, double target, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Random-crop resampler of the patch discriminator (SURVEY.md §8 f1).  Replaces

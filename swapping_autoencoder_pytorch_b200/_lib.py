@@ -12,8 +12,11 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsae_b200.so")
 CSRC_DIR = os.path.join(_HERE, "csrc")
 
-SAE_ABI_VERSION = 19
+SAE_ABI_VERSION = 20
 SAE_STATS_BLOCKS = 128          # header: partials workspace rows of sae_sumsq / sae_adam_norms
+SAE_AUG_UNIFORMS = 21          # header: draws per image of sae_augment_params
+SAE_AUG_NORMALS = 7
+SAE_AUG_RECORD = 32            # header: floats per image record (G_inv, C)
 SAE_E_UNSUPPORTED = -3        # a valid request no kernel of this build takes (header: SAE_E_*)
 
 c_float_p = ctypes.c_void_p   # raw device pointers travel as integers
@@ -126,6 +129,13 @@ SIGNATURES = {
     "sae_adam_norms": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int] + [c_float_p] * 3 + [ctypes.c_float] * 4
                        + [ctypes.c_void_p] * 5 + [c_stream]),
     "sae_score_stats": (ctypes.c_int, [c_float_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, c_stream]),
+    "sae_augment_params": (ctypes.c_int, [c_float_p] * 4 + [ctypes.c_int] * 3 + [c_stream]),
+    "sae_augment_sample": (ctypes.c_int, [c_float_p] * 3 + [ctypes.c_int] * 3 + [ctypes.c_int64] * 4 + [ctypes.c_int, c_stream]),
+    "sae_augment_sample_adjoint": (ctypes.c_int, [c_float_p] * 4 + [ctypes.c_int] * 4 + [c_stream]),
+    "sae_augment_color": (ctypes.c_int, [c_float_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_int64] * 4 + [ctypes.c_int] * 2
+                          + [c_stream]),
+    "sae_augment_color_adjoint": (ctypes.c_int, [c_float_p] * 3 + [ctypes.c_int] * 3 + [ctypes.c_int64] * 4 + [c_stream]),
+    "sae_ada_adjust": (ctypes.c_int, [c_float_p, ctypes.c_void_p, ctypes.c_double, ctypes.c_double, c_stream]),
     "sae_crop_gather": (ctypes.c_int, [c_float_p] * 5 + [ctypes.c_int] * 7 + [ctypes.c_int64] * 4 + [ctypes.c_int, c_stream]),
     "sae_crop_gather_backward": (ctypes.c_int, [c_float_p] * 5 + [ctypes.c_int] * 6 + [ctypes.c_int64] * 4 + [c_stream]),
     "sae_torgb_forward": (ctypes.c_int, [c_float_p] * 5 + [ctypes.c_int] * 4 + [ctypes.c_float, ctypes.c_int, c_stream]),

@@ -232,10 +232,10 @@ class CudaKernels:
         return hi, lo
 
     # ------------------------------------------------------------------ FIR
-    def upfirdn2d(self, x, kernel, up_x, up_y, down_x, down_y, pad_x0, pad_x1, pad_y0, pad_y1, taps=None):
+    def upfirdn2d(self, x, kernel, up_x, up_y, down_x, down_y, pad_x0, pad_x1, pad_y0, pad_y1, taps=None, round_tf32=None):
         """taps: optional host-side 1-D factors (taps_y, taps_x) with kernel == outer(taps_y, taps_x); supplied by
         the Blur modules, which build their kernels from 1-D tap lists — selects the separable fast path wherever that
-        kernel takes the shape."""
+        kernel takes the shape.  round_tf32: override of the rounding policy (the augmentation passes False)."""
         _need_cuda(x, kernel)
         n, h, w, c = x.shape
         kh, kw = kernel.shape
@@ -245,10 +245,10 @@ class CudaKernels:
         pads = (pad_x0, pad_x1, pad_y0, pad_y1)
         if taps is not None and up_x == up_y and down_x == down_y and (len(taps[0]), len(taps[1])) == (kh, kw):
             if self._launch(x.device, "sae_upfirdn2d_separable", _ptr(x), _floats(taps[0]), _floats(taps[1]), _ptr(out), n, h, w,
-                            c, kh, kw, up_x, down_x, *pads, self._round(), refusable=True) != _lib.SAE_E_UNSUPPORTED:
+                            c, kh, kw, up_x, down_x, *pads, self._round(round_tf32), refusable=True) != _lib.SAE_E_UNSUPPORTED:
                 return out
         self._launch(x.device, "sae_upfirdn2d", _ptr(x), _ptr(kernel), _ptr(out), n, h, w, c, kh, kw, up_x, up_y, down_x, down_y,
-                     *pads, self._round())
+                     *pads, self._round(round_tf32))
         return out
 
     # ------------------------------------------------------------- bias/act
@@ -625,6 +625,82 @@ class CudaKernels:
         shape = (ctypes.c_int64 * x.dim())(*x.shape)
         strides = (ctypes.c_int64 * x.dim())(*x.stride())
         self._launch(acc.device, "sae_score_stats", _ptr(x), x.dim(), shape, strides, _ptr(acc))
+
+    # ----------------------------------------------------------------- augmentation (INTEGRATION §2h)
+    def augment_params(self, u, z, p, h, w):
+        """per-image records [N, SAE_AUG_RECORD] (G_inv, then C) from the draws u [N, SAE_AUG_UNIFORMS], z [N, SAE_AUG_NORMALS]
+        and the one-element device probability p, for images of h x w (sae_augment_params)"""
+        _need_cuda(u, z, p)
+        n = u.shape[0]
+        if tuple(u.shape) != (n, _lib.SAE_AUG_UNIFORMS) or tuple(z.shape) != (n, _lib.SAE_AUG_NORMALS):
+            raise _lib.SaeError("augment_params: draws must be [N, %d] and [N, %d]" % (_lib.SAE_AUG_UNIFORMS, _lib.SAE_AUG_NORMALS))
+        rec = torch.empty((n, _lib.SAE_AUG_RECORD), device=u.device, dtype=u.dtype)
+        self._launch(u.device, "sae_augment_params", _ptr(u), _ptr(z), _ptr(p), _ptr(rec), n, h, w)
+        return rec
+
+    def _need_rec(self, rec, n):
+        _need_cuda(rec)
+        if tuple(rec.shape) != (n, _lib.SAE_AUG_RECORD):
+            raise _lib.SaeError("augmentation records must be [N, %d]" % _lib.SAE_AUG_RECORD)
+
+    def augment_sample(self, x, rec, copy_identity=True):
+        """x: logical [N, 3, H, W] (any strides) -> NHWC [N, 2(H + 6), 2(W + 6), 4] (channel 3 zero): the transformed sample
+        grid of the reflect-padded, 2x upsampled image (sae_augment_sample)"""
+        _need_cuda(x, strided=True)
+        n, c, h, w = x.shape
+        if c != 3:
+            raise _lib.SaeError("augment_sample: images must have 3 channels")
+        self._need_rec(rec, n)
+        s = torch.empty((n, 2 * (h + 6), 2 * (w + 6), 4), device=x.device, dtype=x.dtype)
+        self._launch(x.device, "sae_augment_sample", _ptr(x), _ptr(rec), _ptr(s), n, h, w, *x.stride(), int(copy_identity))
+        return s
+
+    def augment_sample_adjoint(self, ds, gc, rec, h, w, copy_identity=True):
+        """adjoint of ``augment_sample``: ds NHWC [N, 2(h + 6), 2(w + 6), 4] -> NHWC [N, h, w, 3]; an image whose G_inv is I
+        copies channels 0..2 of gc NHWC [N, h, w, 4] instead (copy_identity)"""
+        _need_cuda(ds, gc)
+        n = ds.shape[0]
+        if tuple(ds.shape) != (n, 2 * (h + 6), 2 * (w + 6), 4) or (gc is not None and tuple(gc.shape) != (n, h, w, 4)):
+            raise _lib.SaeError("augment_sample_adjoint: shape mismatch")
+        self._need_rec(rec, n)
+        dx = torch.empty((n, h, w, 3), device=ds.device, dtype=ds.dtype)
+        self._launch(ds.device, "sae_augment_sample_adjoint", _ptr(ds), _ptr(gc), _ptr(rec), _ptr(dx), n, h, w, int(copy_identity))
+        return dx
+
+    def augment_color(self, a, b, rec, offset=True, copy_identity=True):
+        """NHWC [N, H, W, 3] = C[:3, :3] v (+ C[:3, 3] with offset), v = a (logical [N, 3, H, W], any strides) for an image whose
+        G_inv is I (copy_identity), else channels 0..2 of b (NHWC [N, H, W, 4]) (sae_augment_color)"""
+        _need_cuda(a, strided=True)
+        _need_cuda(b)
+        n, h, w, c = b.shape
+        if c != 4 or tuple(a.shape) != (n, 3, h, w):
+            raise _lib.SaeError("augment_color: shape mismatch")
+        self._need_rec(rec, n)
+        out = torch.empty((n, h, w, 3), device=b.device, dtype=b.dtype)
+        self._launch(b.device, "sae_augment_color", _ptr(a), _ptr(b), _ptr(rec), _ptr(out), n, h, w, *a.stride(), int(offset),
+                     int(copy_identity))
+        return out
+
+    def augment_color_adjoint(self, dy, rec):
+        """dy: logical [N, 3, H, W] (any strides) -> NHWC [N, H, W, 4] = C[:3, :3]^T dy, channel 3 zero
+        (sae_augment_color_adjoint)"""
+        _need_cuda(dy, strided=True)
+        n, c, h, w = dy.shape
+        if c != 3:
+            raise _lib.SaeError("augment_color_adjoint: images must have 3 channels")
+        self._need_rec(rec, n)
+        gc = torch.empty((n, h, w, 4), device=dy.device, dtype=dy.dtype)
+        self._launch(dy.device, "sae_augment_color_adjoint", _ptr(dy), _ptr(rec), _ptr(gc), n, h, w, *dy.stride())
+        return gc
+
+    def ada_adjust(self, p, acc, step, target):
+        """p = max(0, p + (float)(sign(acc[1] / acc[2] - target) * step)) when acc[2] > 0, then acc = 0 (sae_ada_adjust).
+        p: one-element fp32 device tensor; acc: the four fp64 sums of ``score_stats``"""
+        _need_cuda(p)
+        _need_fp64(acc)
+        if p.numel() != 1 or acc.numel() != 4:
+            raise _lib.SaeError("ada_adjust: p needs one element and acc four")
+        self._launch(p.device, "sae_ada_adjust", _ptr(p), _ptr(acc), float(step), float(target))
 
     # ----------------------------------------------------------------- ToRGB
     def torgb_forward(self, x, s, w, bias, wscale):

@@ -21,6 +21,8 @@ images copied into a static input buffer.
   step of the ramp.
 * Training statistics (opt.training_stats): the score launches sit in the model's forward and the norm launches follow
   the Adam update wherever that runs; both add into a window that lives outside the pool.
+* Augmentation (opt.augment_p / opt.ada_target): the draws, the record launch and the operator sit in the model's forward;
+  p and the sign sums live outside the pool, and the tuning launch runs eagerly after the D replay.
 * A body that fails to capture falls back to eager execution for the rest of the run (``self.disabled`` holds why).
 """
 import gc
@@ -39,8 +41,8 @@ class HalfStepGraphs:
         self.warmup = warmup
         self.calls = {}
         # (kind, input shape, kernel precision, deterministic, non-finite guard[, micro-batches when > 1][, the average's
-        # setting for G when it is on][, ("stats",) when the statistics are on]) -> (graph, static_input, static_outputs,
-        # launches, ...)
+        # setting for G when it is on][, ("stats",) when the statistics are on][, ("ada",) when the augmentation is on]) ->
+        # (graph, static_input, static_outputs, launches, ...)
         self.captured = {}
         self.pool = None
         self.stream = None             # side stream shared by the eager warm-up calls and every capture (see _side)
@@ -124,6 +126,7 @@ class HalfStepGraphs:
         if kind == "G":
             extra += self.trainer.ema_key()                # () with the average off
         extra += self.trainer.stats_key()                  # () with the statistics off
+        extra += self.trainer.augment_key()                # () with the augmentation off
         n = self.calls.get((kind, precision, det, guard) + extra, 0)
         self.calls[(kind, precision, det, guard) + extra] = n + 1
         key = (kind, tuple(images.shape), precision, det, guard) + extra

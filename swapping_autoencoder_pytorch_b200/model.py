@@ -113,6 +113,11 @@ class SwappingAutoencoderModel(BaseModel):
     # that is handed every discriminator logit tensor of the D ("D") and G ("G") losses, R1 aside (optimizer.TrainingStats).
     # It only reads them: losses and random draws are the same with and without it.
     score_sink = None
+    # adaptive discriminator augmentation (extension, opt.augment_p / opt.ada_target): the trainer sets this to its
+    # augment.AugmentPipe.  Every input of D is then augmented — one draw per loss evaluation for all the images D sees, in
+    # the order real, rec, mix, so batched and three-pass discriminators see the same images — and the D step hands the
+    # logits of the augmented reals to ``observe``.  Dpatch's crops are not augmented.
+    augment_pipe = None
 
     @staticmethod
     def modify_commandline_options(parser, is_train):
@@ -163,12 +168,20 @@ class SwappingAutoencoderModel(BaseModel):
         lam = self.opt.lambda_GAN
         if lam == 0.0:
             return {}
+        sizes = [real.size(0), rec.size(0), mix.size(0)]
         if getattr(self.opt, "batch_discriminator_passes", False):
             # extension: D has no cross-sample operation, so one pass over the concatenated batch gives the same
             # per-sample predictions with a third of the launches and fuller tiles on the small late layers
-            pred_real, pred_rec, pred_mix = self.D(torch.cat([real, rec, mix])).split([real.size(0), rec.size(0), mix.size(0)])
+            x = torch.cat([real, rec, mix])
+            if self.augment_pipe is not None:
+                x = self.augment_pipe(x)
+            pred_real, pred_rec, pred_mix = self.D(x).split(sizes)
         else:
+            if self.augment_pipe is not None:
+                real, rec, mix = self.augment_pipe(torch.cat([real, rec, mix])).split(sizes)
             pred_real, pred_rec, pred_mix = self.D(real), self.D(rec), self.D(mix)
+        if self.augment_pipe is not None:
+            self.augment_pipe.observe(pred_real)
         if self.score_sink is not None:
             for name, pred in (("real", pred_real), ("rec", pred_rec), ("mix", pred_mix)):
                 self.score_sink("D", name, pred)
@@ -231,7 +244,8 @@ class SwappingAutoencoderModel(BaseModel):
         penalty = 0.0
         if opt.lambda_R1 > 0.0:
             real.requires_grad_()
-            pred = self.D(real).sum()
+            # with augmentation the penalty is the gradient of D(aug(real)) with respect to the un-augmented real (ADA)
+            pred = self.D(real if self.augment_pipe is None else self.augment_pipe(real)).sum()
             g, = torch.autograd.grad(outputs=pred, inputs=[real], create_graph=True, retain_graph=True)
             penalty = g.pow(2).sum(list(range(1, g.ndim))) * (opt.lambda_R1 * 0.5)
         crop_penalty = 0.0
@@ -263,10 +277,17 @@ class SwappingAutoencoderModel(BaseModel):
             real, gl, sp_mix = real[b // 2:], gl[b // 2:], sp_mix[b // 2:]
         mix = self.G(sp_mix, gl)
         if opt.lambda_GAN > 0.0:
+            sizes = [rec.size(0), mix.size(0)]
             if getattr(opt, "batch_discriminator_passes", False):
-                pred_rec, pred_mix = self.D(torch.cat([rec, mix])).split([rec.size(0), mix.size(0)])
+                x = torch.cat([rec, mix])
+                if self.augment_pipe is not None:
+                    x = self.augment_pipe(x)
+                pred_rec, pred_mix = self.D(x).split(sizes)
             else:
-                pred_rec, pred_mix = self.D(rec), self.D(mix)
+                d_rec, d_mix = rec, mix
+                if self.augment_pipe is not None:
+                    d_rec, d_mix = self.augment_pipe(torch.cat([rec, mix])).split(sizes)
+                pred_rec, pred_mix = self.D(d_rec), self.D(d_mix)
             if self.score_sink is not None:
                 self.score_sink("G", "rec", pred_rec)
                 self.score_sink("G", "mix", pred_mix)

@@ -10,7 +10,7 @@ import os
 
 import torch
 
-from . import _lib, backend, util
+from . import _lib, augment, backend, util
 
 
 class MultiTensorAdam:
@@ -279,6 +279,15 @@ class SwappingAutoencoderOptimizer:
         parser.add_argument("--training_stats", type=util.str2bool, nargs="?", const=True, default=False,
                             help="training statistics (extension): accumulate per-update gradient, weight and Adam-step norms "
                                  "and the discriminators' scores on the device; read them with trainer.training_stats()")
+        parser.add_argument("--augment_p", default=0.0, type=float,
+                            help="adaptive discriminator augmentation (extension): probability of each transform of D's inputs; "
+                                 "the initial value when --ada_target > 0")
+        parser.add_argument("--ada_target", default=0.0, type=float,
+                            help="tune the augmentation probability on the device towards E[sign(D(real))] = this value "
+                                 "(StyleGAN2-ADA uses 0.6); 0: no tuning")
+        parser.add_argument("--ada_kimg", default=500.0, type=float,
+                            help="thousands of images over which the tuned probability can move by one")
+        parser.add_argument("--ada_interval", default=4, type=int, help="tune the probability every this many D updates")
         return parser
 
     def __init__(self, model):
@@ -326,6 +335,16 @@ class SwappingAutoencoderOptimizer:
             inner = self._inner()
             if hasattr(inner, "score_sink"):    # this package's model; the reference's own model file has no sink
                 inner.score_sink = self.stats.score
+        # adaptive discriminator augmentation (extension, ``opt.augment_p`` > 0 or ``opt.ada_target`` > 0): p and the sign
+        # sums live outside any graph pool, like the shadow
+        self.augment = None
+        ada = (float(getattr(opt, "augment_p", 0.0)), float(getattr(opt, "ada_target", 0.0)),
+               float(getattr(opt, "ada_kimg", 500.0)), getattr(opt, "ada_interval", 4))
+        if augment.check_options(*ada) and self.Gparams:
+            self.augment = augment.AugmentPipe(*ada, self.Gparams[0].device, world=self.world)
+            inner = self._inner()
+            if hasattr(inner, "augment_pipe"):  # this package's model; the reference's own model file has no hook
+                inner.augment_pipe = self.augment
 
     def _inner(self):
         return getattr(self.model, "singlegpu_model", self.model)
@@ -337,6 +356,16 @@ class SwappingAutoencoderOptimizer:
     def stats_key(self):
         """what a captured graph bakes in of the statistics: () when they are off, so the graph keys stay as they were"""
         return () if self.stats is None else (("stats",),)
+
+    def augment_key(self):
+        """what a captured graph bakes in of the augmentation: () when it is off, so the graph keys stay as they were"""
+        return () if self.augment is None else (("ada",),)
+
+    def augment_p(self):
+        """the current augmentation probability p (opt.augment_p, tuned with opt.ada_target > 0); one device-to-host read"""
+        if self.augment is None:
+            raise RuntimeError("no augmentation: opt.augment_p and opt.ada_target are 0")
+        return self.augment.value()
 
     def training_stats(self, reset=True, per_tensor=False):
         """The statistics accumulated since the last reset (opt.training_stats; INTEGRATION.md §2g), as plain floats, with
@@ -561,6 +590,11 @@ class SwappingAutoencoderOptimizer:
         if needs_r1:
             d_losses.update(self._run("R1", images))
 
+        if self.augment is not None and self.augment.tuning() and self.discriminator_iter_counter % self.augment.interval == 0:
+            # every ada_interval-th D update: fold the sign sums of D(aug(real)) into p (one launch, eager: the captured
+            # D graph is the same on adjusting and non-adjusting steps)
+            self.augment.adjust(images.shape[0])
+
         d_losses["D_total"] = sum(v.mean() for v in d_losses.values())
         d_losses.update(d_metrics)
         return d_losses
@@ -574,13 +608,16 @@ class SwappingAutoencoderOptimizer:
         """Adam state of both groups (torch.optim.Adam's format) + the schedule counters.  The reference never saves this
         (optimizers/base_optimizer.py has no state I/O): resuming there restarts Adam's moments from zero.  With
         ``opt.skip_nonfinite_steps`` the guard's skip counters (``nonfinite_steps()``) are saved as well, with ``opt.ema_kimg``
-        > 0 the weight average under "ema" (``ParameterEMA.state_dict``: the shadow by state_dict key, and t)."""
+        > 0 the weight average under "ema" (``ParameterEMA.state_dict``: the shadow by state_dict key, and t), with the
+        augmentation on its probability and sign sums under "ada" ({"p", "acc"})."""
         sd = {"optimizer_G": self.optimizer_G.state_dict(), "optimizer_D": self.optimizer_D.state_dict(),
               "train_mode_counter": self.train_mode_counter, "discriminator_iter_counter": self.discriminator_iter_counter}
         if self.nonfinite_guard_on():
             sd["nonfinite_steps"] = self.nonfinite_steps()
         if self.ema is not None:
             sd["ema"] = self.ema.state_dict()
+        if self.augment is not None:
+            sd["ada"] = self.augment.state_dict()
         return sd
 
     def load_state_dict(self, sd):
@@ -593,6 +630,8 @@ class SwappingAutoencoderOptimizer:
             self._nonfinite_counters().copy_(torch.tensor(counts, dtype=torch.int64))     # in place: captured graphs hold it
         if self.ema is not None and "ema" in sd:
             self.ema.load_state_dict(sd["ema"])          # without one the construction-time copy stays
+        if self.augment is not None and "ada" in sd:
+            self.augment.load_state_dict(sd["ada"])      # in place: captured graphs hold p and the sign sums
 
     def _optimizer_path(self, total_steps_so_far=None, what="optimizer"):
         name = "latest_%s.pth" % what if total_steps_so_far is None else "%dk_%s.pth" % (total_steps_so_far // 1000, what)

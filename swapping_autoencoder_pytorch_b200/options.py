@@ -54,6 +54,11 @@ def default_options(**overrides):
         # sign of every discriminator logit tensor, accumulated on the device until trainer.training_stats() reads them
         # (optimizer.TrainingStats; INTEGRATION.md §2g)
         training_stats=False,
+        # extension: adaptive discriminator augmentation — StyleGAN2-ADA's geometric and colour transforms of every input of D
+        # with probability augment_p; ada_target > 0 tunes it on the device towards E[sign(D(real))] = ada_target, moving it
+        # by up to one unit per ada_kimg thousand images, every ada_interval D updates; on iff augment_p > 0 or ada_target > 0
+        # (augment.AugmentPipe; INTEGRATION.md §2h)
+        augment_p=0.0, ada_target=0.0, ada_kimg=500.0, ada_interval=4,
     )
     for k, v in overrides.items():
         setattr(opt, k, v)
